@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""bench.py — BGZF inflate (+ CRAM rANS-Nx16 decode) throughput on B200, beside the reference's
-CPU path on the same box.  Contract: see the task statement / DESIGN.md §Measurement.
+"""bench.py — BGZF inflate (+ CRAM rANS-Nx16 decode) throughput on H100, beside the reference's
+CPU path on the same machine.  See DESIGN.md §Measurement.
 
 One "step" = one pass of the BGZF inflate hot path over the whole synthetic 150 bp BAM
 (BASELINE.json configs[1]: 10 GB uncompressed, zlib level 6, one warp per 64 KiB block).
@@ -11,6 +11,12 @@ One "step" = one pass of the BGZF inflate hot path over the whole synthetic 150 
   cpu_baseline  the unmodified reference (oracle/_ref/libhts_ref.so: bgzf_read + bgzf_mt thread
              pool) on the host cores, on a bounded sample of the same file
   extra.rans CRAM 3.1 rANS-Nx16 decode (BASELINE.json configs[2]) measured after the timed steps
+
+--dump-outputs DIR writes what the last timed step computed, for comparing two builds output for output:
+  block_len.npy, block_status.npy   per BGZF block: inflated length and status (float64)
+  inflated_sample.npy               DUMP_SAMPLE bytes of the inflated stream (float32) at positions drawn
+                                    with numpy default_rng(0).integers(0, uncompressed bytes), sorted
+The corpus is generated from fixed seeds, so the same arguments give the same inputs on every run.
 """
 import argparse
 import ctypes as C
@@ -43,40 +49,31 @@ def parse():
     ap.add_argument("--cpu-sample-gb", type=float, default=4.0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as .npy files to DIR")
     return ap.parse_args()
 
 
-def ncu_traffic(kernel_tag):
-    """dram__bytes_read+write of one launch from the committed ncu --set full capture (profiles/),
-    with the algorithmic bytes of THAT captured launch, so the ratio can be applied honestly."""
-    p = os.path.join(ROOT, "profiles", "r2_%s_ncu_summary.txt" % kernel_tag)
-    if not os.path.exists(p):
-        return None
-    alg = None
-    tp = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    if os.path.exists(tp):
-        alg = json.load(open(tp)).get(kernel_tag, {}).get("algorithmic_bytes")
-    rd = wr = None
-    for line in open(p):
-        f = line.split()
-        if len(f) >= 3 and f[0] == "dram__bytes_read.sum" and rd is None: rd = (float(f[1]), f[2])
-        if len(f) >= 3 and f[0] == "dram__bytes_write.sum" and wr is None: wr = (float(f[1]), f[2])
-    if not rd or not wr:
-        return None
-    scale = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}
-    return {"dram_bytes": rd[0] * scale.get(rd[1], 1) + wr[0] * scale.get(wr[1], 1), "algorithmic_bytes": alg,
-            "source": os.path.relpath(p, ROOT)}
+DUMP_SAMPLE = 12 << 20                  # 48 MB of float32: the whole dump stays under 64 MB
+
+
+def dump_outputs(out_dir, torch, d_out, U, d_len, d_st):
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "block_len.npy"), d_len.cpu().numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, "block_status.npy"), d_st.cpu().numpy().astype(np.float64))
+    pos = np.sort(np.random.default_rng(0).integers(0, U, size=min(U, DUMP_SAMPLE)))
+    idx = torch.from_numpy(pos).to(d_out.device)
+    np.save(os.path.join(out_dir, "inflated_sample.npy"), d_out[idx].cpu().numpy().astype(np.float32))
 
 
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, index):
@@ -210,17 +207,26 @@ def rans_legs(args, ctx, torch, dev, world, dist):
     UNMODIFIED reference encoder (tools/rans_bench.py), NovaSeq 4-bin and HiSeq ~40-value qualities, every
     block compared on the device with the generator's input; device time, host-buffer (e2e) time and the
     reference decoder on the host cores beside it.  Runs at every N (slices shard without a collective)."""
+    import gc
+    import htslib_b200 as H
     from tools import rans_bench
     if args.rans_slices == 0:
         return None
     waves = -args.rans_slices if args.rans_slices < 0 else 1
     out = {}
     for alphabet in ("novaseq", "hiseq"):
+        # each alphabet on a context of its own, closed afterwards: its device staging (as large as the batch)
+        # is released before the next one, so both fit next to the other legs in 80 GB
+        gc.collect()
+        torch.cuda.empty_cache()
+        rctx = H.Context(dev.index)
         try:
-            out[alphabet] = rans_bench.run(ctx, torch, dev, peaks(), alphabet=alphabet, waves=waves, reps=5, world=world,
+            out[alphabet] = rans_bench.run(rctx, torch, dev, peaks(), alphabet=alphabet, waves=waves, reps=5, world=world,
                                            dist=dist, e2e=not args.no_e2e, cpu=(world == 1 and not args.no_cpu_baseline))
         except Exception as ex:                                   # the headline line must still print
             out[alphabet] = {"error": repr(ex)}
+        finally:
+            rctx.close()
     head = dict(out["novaseq"])
     head["hiseq"] = out["hiseq"]
     head["note"] = ("top level = NovaSeq 4-bin qualities (SURVEY.md 8d first data set); 'hiseq' = the 40-value data set; "
@@ -387,6 +393,8 @@ def run_ours(args):
         dist.barrier()
     clocks = sampler.stop() if rank == 0 else None
     ms_step = ms_total / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, torch, d_out, U, d_len, d_st)
 
     # ---- BAM record unpack over the inflated stream, still on the device (configs[3] front half) ----
     bam_extra = None
@@ -574,12 +582,8 @@ def run_ours(args):
         return
     hbm, how = peaks()
     achieved = (U + Cb) / ms_step / 1e6
-    # roofline.traffic: the ncu --set full capture of this kernel on this very workload (same seeds, same launch shape);
-    # only quoted per launch when the captured launch moved the same algorithmic bytes as the timed one
-    cap = ncu_traffic("inflate")
-    traffic = cap["dram_bytes"] if cap and cap.get("algorithmic_bytes") and abs(cap["algorithmic_bytes"] - (U + Cb)) <= 0.01 * (U + Cb) else None
     out = {
-        "metric": "BGZF inflate + CRAM rANS decode GB/s at 1/2/4/8 B200 vs reference CPU",
+        "metric": "BGZF inflate + CRAM rANS decode GB/s at 1/2/4/8 H100 vs reference CPU",
         "value": U * world / ms_step / 1e6, "unit": "GB/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "u8", "data": "synthetic",
@@ -587,18 +591,13 @@ def run_ours(args):
                                % (U / 1e9, args.quals, args.level),
                    "blocks_per_gpu": nb, "uncompressed_bytes_per_gpu": U, "compressed_bytes_per_gpu": Cb,
                    "value_is": "uncompressed bytes / kernel time (inputs resident in HBM)",
-                   "l2_policy": "inputs larger than L2 (%.1f GB in + %.1f GB out per step vs 126 MB)" % (Cb / 1e9, U / 1e9),
+                   "l2_policy": "inputs larger than L2 (%.1f GB in + %.1f GB out per step vs 50 MB)" % (Cb / 1e9, U / 1e9),
                    "data_gen_s": round(corpus["gen_s"], 1), "unique_data": "all blocks unique" if corpus["tile"] == 1 else
                                    "%.2f GB unique per GPU repeated %dx at distinct addresses (host cores shared by %d generators)"
                                    % (U / 1e9 / corpus["tile"], corpus["tile"], world)},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm,
-                     "traffic": traffic, "kernel": "bgzf_inflate_kernel", "algorithmic_bytes_per_launch": U + Cb,
-                     "peak_source": how,
-                     "traffic_note": "dram__bytes_read.sum + dram__bytes_write.sum of one launch from the committed ncu --set full capture of "
-                                     "`python bench.py --gb 10` (profiles/r2_inflate_ncu_summary.txt); null when this run's launch is a different size. "
-                                     "3.6x the algorithmic bytes: the 8-byte match records make a DRAM round trip (~14 GB) and the CRC pass re-reads "
-                                     "the output (~9.7 GB) because 21 warps/SM x (64 KiB window + records) exceeds the 126 MB L2 (DESIGN.md 6)",
-                     "traffic_capture": cap},
+                     "traffic": None, "kernel": "bgzf_inflate_kernel", "algorithmic_bytes_per_launch": U + Cb,
+                     "peak_source": how},
         "gpu_launches": int(launches),
         "clocks": clocks,
     }
@@ -709,7 +708,7 @@ def run_reference(args):
     sample = "first %d BGZF blocks (%.2f GB uncompressed) of the same synthetic BAM per step; unmodified htslib bgzf_read over bgzf_mt(%d), zlib arm (no libdeflate here)" % (nb, ubytes / 1e9, cores)
     print(json.dumps({
         "impl": "reference",
-        "metric": "BGZF inflate + CRAM rANS decode GB/s at 1/2/4/8 B200 vs reference CPU",
+        "metric": "BGZF inflate + CRAM rANS decode GB/s at 1/2/4/8 H100 vs reference CPU",
         "value": v, "unit": "GB/s", "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": sec * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "u8", "data": "synthetic",

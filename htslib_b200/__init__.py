@@ -1,4 +1,4 @@
-"""htslib_b200 — Python face of libhtsgpu.so (hand-written sm_100a CUDA behind a C ABI).
+"""htslib_b200 — Python face of libhtsgpu.so (hand-written sm_90a CUDA behind a C ABI).
 
 The library is the product; this module only loads it with ctypes and passes raw pointers
 (torch is used by callers for device memory and streams, never for compute).  There is no CPU

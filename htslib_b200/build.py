@@ -1,4 +1,4 @@
-"""Builds htslib_b200/libhtsgpu.so in-tree with nvcc for sm_100a (no torch involved)."""
+"""Builds htslib_b200/libhtsgpu.so in-tree with nvcc for sm_90a (no torch involved)."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, os.environ.get("HGPU_OUT", "libhtsgpu.so"))      # HGPU_OUT: side-by-side tuning builds
 BUILD = os.path.join(HERE, os.environ.get("HGPU_BUILD_DIR", "build"))
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "--use_fast_math", "-Xptxas", "-v"]
 FLAGS += os.environ.get("HGPU_DEFS", "").split()
 if os.environ.get("HGPU_PROFILE"):
@@ -50,7 +50,7 @@ def build(force=False, verbose=False):
         f.write("\n".join(log))
     if verbose:
         sys.stderr.write("\n".join(log))
-    cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static", "-lpthread", "-ldl", "-lrt"]
+    cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart_static", "-lpthread", "-ldl", "-lrt"]
     subprocess.check_call(cmd)
     return OUT
 

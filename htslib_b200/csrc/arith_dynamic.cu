@@ -1,4 +1,4 @@
-// Adaptive arithmetic coder ("ARITH_PR", CRAM 3.1 block method 6) decoder for sm_100a.
+// Adaptive arithmetic coder ("ARITH_PR", CRAM 3.1 block method 6) decoder for sm_90a.
 //
 // Replaces arith_uncompress_to and the bodies behind it (htscodecs arith_dynamic.c:1033-1278,
 // :137-165 O0, :227-272 O1, :520-580 O0_RLE, :660-728 O1_RLE; range coder c_range_coder.h:62-166;

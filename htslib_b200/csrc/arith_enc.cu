@@ -1,4 +1,4 @@
-// Adaptive arithmetic coder ("ARITH_PR", CRAM 3.1 block method 6) ENCODER for sm_100a.
+// Adaptive arithmetic coder ("ARITH_PR", CRAM 3.1 block method 6) ENCODER for sm_90a.
 //
 // Stands where arith_compress_to stands (htscodecs/htscodecs/arith_dynamic.c:730-1026) with the bodies
 // behind it: arith_compress_O0 :98-136, _O1 :172-222, _O0_RLE :441-519, _O1_RLE :572-658, hts_pack

@@ -1,4 +1,4 @@
-// BAM record unpack for sm_100a: the data movement of bam_read1 (htslib sam.c:784-860) plus the
+// BAM record unpack for sm_90a: the data movement of bam_read1 (htslib sam.c:784-860) plus the
 // 4-bit SEQ expand and QUAL+33 of sam_format1_append (sam.c:4324-4404; nibble2base,
 // sam_internal.h:63-118; add33, sam.c:4317-4322), over an inflated BAM record stream that is
 // already resident in device memory (the output of the BGZF inflate kernel).

@@ -1,4 +1,4 @@
-// BGZF block inflate for sm_100a: one warp per <=64 KiB BGZF block.
+// BGZF block inflate for sm_90a: one warp per <=64 KiB BGZF block.
 //
 // Replaces, for a batch of blocks, what one htslib worker does per job in bgzf_decode_func
 // (bgzf.c:1373-1384): check_header (:896-903), inflate_block (:808-824) -> bgzf_uncompress
@@ -626,9 +626,9 @@ constexpr uint32_t MREC_CAP = 65536 / 3 + 64;   // a match yields >= 3 bytes of 
 
 // Parallel decode of one Huffman block body starting at bit `body` of the member (bit 0 = first
 // bit of word wbase[0], i.e. positions include the alignment offset).  total = end of input.
-// A/B on B200 (tools/prof_inflate.py, profiles/r2_inflate_ab.txt): for the warp kernel the register-buffered bit reader
-// below beats the position-based branch-free walk of bgzf_huff.cuh (its two stream loads per symbol come from global
-// memory here, not from a staged copy), and 5 warps per CTA (20 per SM) are no faster than 4.  -DHGPU_NEW_WALK selects the other.
+// The warp kernel uses the register-buffered bit reader below rather than the position-based branch-free walk of
+// bgzf_huff.cuh, whose two stream loads per symbol come from global memory here, not from a staged copy.
+// -DHGPU_NEW_WALK selects the other (A/B with tools/prof_inflate.py).
 #ifndef HGPU_NEW_WALK
 __device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const uint32_t *wend, uint32_t body,
                                     uint32_t total, uint8_t *out, uint32_t cap, uint32_t &o, uint2 *mrec,
@@ -1486,9 +1486,9 @@ int hgpu_launch_bgzf_inflate(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t 
     if (hgpu_check(cudaSetDevice(ctx->device), "cudaSetDevice")) return HGPU_ERR_CUDA;
     int rc = ensure_crc_tables(ctx, st);
     if (rc) return rc;
-    // The product path is the warp-per-block kernel (21 blocks in flight per SM, LZ77 through L2 with
-    // per-lane word copies: 232 GB/s on sorted BAM).  HGPU_INFLATE_CTA=1 selects the CTA-per-block kernel
-    // (window in shared memory, 2 blocks per SM: 127 GB/s) for A/B measurements.
+    // The product path is the warp-per-block kernel (as many blocks in flight per SM as occupancy allows,
+    // LZ77 through L2 with per-lane word copies).  HGPU_INFLATE_CTA=1 selects the CTA-per-block kernel
+    // (window in shared memory, 2 blocks per SM) for A/B measurements.
     static const bool use_warp = !(getenv("HGPU_INFLATE_CTA") && getenv("HGPU_INFLATE_CTA")[0] == '1');
     static bool attr_set[64];                          // function attributes are per device
     const int dv = ctx->device & 63;

@@ -34,7 +34,7 @@ int hgpu_check(cudaError_t e, const char *what)
 void hgpu_count_launch(int n) { g_launches += (uint64_t)n; }
 
 extern "C" const char *hgpu_last_error(void) { return g_err; }
-extern "C" const char *hgpu_version(void) { return "htsgpu 0.1 (sm_100a)"; }
+extern "C" const char *hgpu_version(void) { return "htsgpu 0.1 (sm_90a)"; }
 extern "C" uint64_t hgpu_launch_count(void) { return g_launches.load(); }
 
 static int grow(uint8_t **p, size_t *cap, size_t want, bool pinned)

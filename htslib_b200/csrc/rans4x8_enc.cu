@@ -1,4 +1,4 @@
-// rANS 4x8 ("RANS", CRAM 3.0 block method 4) ENCODER for sm_100a.
+// rANS 4x8 ("RANS", CRAM 3.0 block method 4) ENCODER for sm_90a.
 //
 // Stands where rans_compress stands (htscodecs/htscodecs/rANS_static.c:829-838) with rans_compress_O0
 // (:75-214) and rans_compress_O1 (:387-597) behind it.  CRAM 3.0 is the legacy write path, so this is the

@@ -1,4 +1,4 @@
-// rANS Nx16 ("RANS_PR", CRAM 3.1 block method 5) decoder for sm_100a.
+// rANS Nx16 ("RANS_PR", CRAM 3.1 block method 5) decoder for sm_90a.
 //
 // Replaces rans_uncompress_to_4x16 and the four symbol loops behind it
 // (htscodecs rANS_static4x16pr.c:1586-1873, :213-328, :504-800; rANS_static32x16pr.c:254-408,
@@ -8,7 +8,7 @@
 // which is exactly the "states renormalise in index order" rule of the scalar code
 // (rANS_static32x16pr.c:334-337, :657-666).
 //
-// Table layout (B200-first, not the reference's): per context row a BYTE lookup
+// Table layout (GPU-first, not the reference's): per context row a BYTE lookup
 //   lut[row][m] -> compact symbol index       (1<<shift bytes)
 // plus a small per-(row,symbol) record
 //   fb[row][k]  -> { f | start<<16 , byte }   (8 bytes)

@@ -1,4 +1,4 @@
-// rANS Nx16 ("RANS_PR", CRAM 3.1 method 5) ENCODER for sm_100a — order 0 / order 1, 4-way or
+// rANS Nx16 ("RANS_PR", CRAM 3.1 method 5) ENCODER for sm_90a — order 0 / order 1, 4-way or
 // 32-way (X32), PACK, RLE, STRIPE (with the per-part method trial) and the CAT fallback; one warp per stream.
 //
 // Stands where rans_compress_to_4x16 -> rans_compress_O0/O1_4x16 / _32x16 stand in the reference

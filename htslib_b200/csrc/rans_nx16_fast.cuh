@@ -408,7 +408,7 @@ __device__ __forceinline__ void fast32_stream(const FastJob *fj, uint32_t lut_a,
     __syncwarp();
 }
 
-// where the dynamic shared window of a CTA starts (the first KiB of the window is the system's on sm_100)
+// where the dynamic shared window of a CTA starts (the system reserves the first KiB of a CTA's shared memory)
 __global__ void rans_smem_probe_kernel(uint32_t *o)
 {
     extern __shared__ __align__(16) uint8_t smem[];

@@ -1,5 +1,5 @@
 /*
- * htsgpu.h — C ABI of libhtsgpu.so, the B200 (sm_100a) implementation of htslib's
+ * htsgpu.h — C ABI of libhtsgpu.so, the H100 (sm_90a) implementation of htslib's
  * compression/decode hot path.  Plain pointers and sizes only; no torch / C++ types.
  *
  * Two layers:

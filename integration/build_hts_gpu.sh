@@ -14,13 +14,14 @@
 #   * everything else is compiled from /root/reference where it lies, exactly as oracle/build_ref.sh
 #     does for the stock build.
 #
-# Output (git-ignored, travels to the GPU box): integration/_build/libhts_gpu.so and the reference's
-# own test programs linked against it: test_bgzf, test_view, bgzip.
+# Output (git-ignored; under oracle/_ref/ with the stock build, so both travel together):
+# oracle/_ref/integration/libhts_gpu.so and the reference's own test programs linked against it:
+# test_bgzf, test_view, bgzip (and the same three on the stock build in stock/).
 set -euo pipefail
 REF=${REF:-/root/reference}
 HERE=$(cd "$(dirname "$0")" && pwd)
 ROOT=$(dirname "$HERE")
-OUT=$HERE/_build
+OUT=${OUT:-$ROOT/oracle/_ref/integration}
 [ -d "$REF" ] || { echo "no reference tree at $REF; keeping prebuilt $OUT" >&2; exit 0; }
 [ -f "$ROOT/htslib_b200/libhtsgpu.so" ] || { echo "build htslib_b200/libhtsgpu.so first" >&2; exit 1; }
 mkdir -p "$OUT/obj" "$OUT/src"
@@ -50,7 +51,7 @@ for s in $SRCS; do
   fi
 done
 for p in "${pids[@]}"; do wait $p; done
-RP='-Wl,-rpath,$ORIGIN/../../htslib_b200 -Wl,-rpath,$ORIGIN'
+RP='-Wl,-rpath,$ORIGIN/../../../htslib_b200 -Wl,-rpath,$ORIGIN'
 gcc -shared -o "$OUT/libhts_gpu.so" $OBJS -L"$ROOT/htslib_b200" -lhtsgpu $RP -lz -lm -lpthread
 for t in test/test_bgzf test/test_view bgzip; do
   gcc $CFLAGS -o "$OUT/$(basename $t)" "$REF/$t.c" -L"$OUT" -lhts_gpu -L"$ROOT/htslib_b200" -lhtsgpu $RP -lz -lm -lpthread
@@ -59,7 +60,7 @@ done
 if [ -f "$ROOT/oracle/_ref/libhts_ref.so" ]; then
   mkdir -p "$OUT/stock"
   for t in test/test_bgzf test/test_view bgzip; do
-    gcc $CFLAGS -o "$OUT/stock/$(basename $t)" "$REF/$t.c" -L"$ROOT/oracle/_ref" -lhts_ref '-Wl,-rpath,$ORIGIN/../../../oracle/_ref' -lz -lm -lpthread
+    gcc $CFLAGS -o "$OUT/stock/$(basename $t)" "$REF/$t.c" -L"$ROOT/oracle/_ref" -lhts_ref '-Wl,-rpath,$ORIGIN/../..' -lz -lm -lpthread
   done
 fi
 echo "built $OUT/libhts_gpu.so"

@@ -65,3 +65,7 @@ done
 for p in "${pids[@]}"; do wait $p; done
 gcc -shared -o "$OUT/libhts_ref.so" $OBJS -lz -lm -lpthread
 echo "built $OUT/libhts_ref.so"
+# the reference's own test programs around libhtsgpu.so (tests/test_integration.py), once the product is built
+if [ -f "$HERE/../htslib_b200/libhtsgpu.so" ]; then
+  bash "$HERE/../integration/build_hts_gpu.sh"
+fi

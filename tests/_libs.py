@@ -1,17 +1,194 @@
 """ctypes loaders for the three libraries the tests compare.
 
   orc()  -> oracle/liborc.so          CPU restatement (test infrastructure)
-  ref()  -> oracle/_ref/libhts_ref.so unmodified reference, compiled from /root/reference (may be absent)
+  ref()  -> oracle/_ref/libhts_ref.so unmodified reference (htslib + htscodecs), built by oracle/build_ref.sh
+                                      from the reference sources; usually absent
   The product library is loaded through htslib_b200 itself.
+
+Every ref_* helper answers from tests/golden/ref_calls/: what the compiled reference returned for the
+same arguments, recorded once.  So the comparisons with the reference run where the reference was never
+built.  Only results of up to STORE_LIMIT characters are stored (more for the helpers that read or
+write the reference's own fixtures), which keeps the small cases of every test.  Where oracle/_ref is
+absent, a case whose result is not stored is passed over (`with sampled():` around one case of a loop)
+and a test that needs one outside such a block is skipped; where oracle/_ref is built every case runs.
+To store the results of new inputs, build oracle/_ref and run the tests with
+HTS_REF_RECORD=tests/golden/ref_calls.
 """
+import atexit
+import ast
+import contextlib
 import ctypes as C
+import functools
+import gzip
+import hashlib
 import os
 import subprocess
 
+import pytest
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden")
+REF_CALLS = os.path.join(GOLD, "ref_calls")
+STORE_LIMIT = 1500
 u8p = C.POINTER(C.c_uint8)
 _orc = _ref = None
+_stored = {}          # helper name -> {key: repr of the result}
+_used = {}            # helper name -> {key: repr of the result} of every call in this process
+_limit = {}           # helper name -> longest result stored
+_always = set()       # (helper name, key) stored whatever their size: the base streams of the corruption tests
+
+
+def _canon(x, h):
+    """Feed an argument into the key: byte strings and files by content, everything else by repr."""
+    if isinstance(x, (bytes, bytearray, memoryview)):
+        h.update(b"B%d:" % len(x)); h.update(bytes(x))
+    elif isinstance(x, str) and os.path.isfile(x):
+        with open(x, "rb") as f:
+            data = f.read()
+        h.update(b"F%d:" % len(data)); h.update(data)
+    elif isinstance(x, (list, tuple)):
+        h.update(b"L%d[" % len(x))
+        for v in x:
+            _canon(v, h)
+        h.update(b"]")
+    elif hasattr(x, "tolist"):                    # numpy arrays and scalars
+        _canon(x.tolist(), h)
+    elif isinstance(x, (int, float, str, type(None))):
+        h.update(b"V" + repr(x).encode() + b";")
+    else:
+        raise TypeError("reference call argument of type %s" % type(x).__name__)
+
+
+def _load(name):
+    if name not in _stored:
+        d = {}
+        p = os.path.join(REF_CALLS, name + ".gz")
+        if os.path.exists(p):
+            with gzip.open(p, "rt") as f:
+                for line in f:
+                    k, _, v = line.rstrip("\n").partition("\t")
+                    d[k] = v
+        _stored[name] = d
+    return _stored[name]
+
+
+def _flush():
+    """HTS_REF_RECORD=<dir>: add every result this process used to <dir>/<helper>.gz."""
+    out = os.environ.get("HTS_REF_RECORD")
+    if not out or not _used:
+        return
+    os.makedirs(out, exist_ok=True)
+    for name, used in _used.items():
+        d = {}
+        p = os.path.join(out, name + ".gz")
+        if os.path.exists(p):
+            with gzip.open(p, "rt") as f:
+                for line in f:
+                    k, _, v = line.rstrip("\n").partition("\t")
+                    d[k] = v
+        d.update((k, v) for k, v in used.items() if len(v) <= _limit[name] or (name, k) in _always)
+        with open(p, "wb") as raw, gzip.GzipFile(fileobj=raw, mode="wb", compresslevel=9, mtime=0) as f:
+            f.write("".join("%s\t%s\n" % kv for kv in sorted(d.items())).encode())
+
+
+atexit.register(_flush)
+
+
+class Digest:
+    """A byte string the reference returned, kept as its length, the first 64 bits of its SHA-256 and its
+    first bytes: equal to exactly that string.  Stands for decoder outputs, which the tests only compare;
+    strings shorter than MIN (names, short fields) are kept as they are."""
+    HEAD = 4
+    MIN = 64
+
+    def __init__(self, n, sha, head):
+        self.n, self.sha, self.head = n, sha, head
+
+    def __eq__(self, other):
+        if isinstance(other, Digest):
+            return (self.n, self.sha) == (other.n, other.sha)
+        if isinstance(other, (bytes, bytearray, memoryview)):
+            return len(other) == self.n and hashlib.sha256(other).hexdigest()[:16] == self.sha
+        return NotImplemented
+
+    __hash__ = None
+
+    def __len__(self):
+        return self.n
+
+    def __getitem__(self, i):
+        if isinstance(i, int) and 0 <= i < len(self.head):
+            return self.head[i]
+        raise IndexError("only the first %d bytes of a stored decoder output are kept" % self.HEAD)
+
+    def __repr__(self):
+        return "<%d bytes, sha256 %s...>" % (self.n, self.sha)
+
+
+_DIGEST_TAG = "sha256-of-bytes"
+
+
+def _shrink(v):
+    if isinstance(v, (bytes, bytearray)) and len(v) >= Digest.MIN:
+        return (_DIGEST_TAG, len(v), hashlib.sha256(v).hexdigest()[:16], bytes(v[:Digest.HEAD]))
+    if isinstance(v, (list, tuple)):
+        return type(v)(_shrink(x) for x in v)
+    return v
+
+
+def _grow(v):
+    if isinstance(v, tuple) and len(v) == 4 and v[0] == _DIGEST_TAG:
+        return Digest(v[1], v[2], v[3])
+    if isinstance(v, (list, tuple)):
+        return type(v)(_grow(x) for x in v)
+    return v
+
+
+class NotStored(pytest.skip.Exception):
+    """A reference result that is not among the stored ones, with no compiled reference to compute it."""
+
+
+@contextlib.contextmanager
+def sampled():
+    """One case of a loop over inputs: passed over when one of its reference results is not stored."""
+    try:
+        yield
+    except NotStored:
+        pass
+
+
+def stored_reference(fn=None, *, digest=False, limit=STORE_LIMIT):
+    """The result of fn (a call into the compiled reference) for these arguments, from the stored results.
+    fn must return plain values (bytes, str, numbers, None, tuples, lists) and take content-keyed arguments.
+    digest: keep byte strings of the result as Digest (True, or a predicate of the keyword arguments).
+    limit: longest result (characters of its repr) that is stored; a call with store_always=True is stored
+    whatever its size."""
+    if fn is None:
+        return functools.partial(stored_reference, digest=digest, limit=limit)
+    name = fn.__name__
+    _limit[name] = limit
+
+    @functools.wraps(fn)
+    def call(*args, store_always=False, **kw):
+        h = hashlib.sha256(name.encode())
+        _canon(args + tuple(sorted(kw.items())), h)
+        key = h.hexdigest()[:16]
+        if store_always:
+            _always.add((name, key))
+        v = _load(name).get(key) or _used.get(name, {}).get(key)
+        if v is None:
+            if ref() is None:
+                raise NotStored("%s%s: no stored reference result and oracle/_ref not built" % (name, _short(args)))
+            res = fn(*args, **kw)
+            v = repr(_shrink(res) if (digest(kw) if callable(digest) else digest) else res)
+        _used.setdefault(name, {})[key] = v
+        return _grow(ast.literal_eval(v))
+    return call
+
+
+def _short(args):
+    s = repr(tuple(a if not isinstance(a, (bytes, bytearray)) or len(a) < 32 else "<%d bytes>" % len(a) for a in args))
+    return s[:300]
 
 
 def orc():
@@ -26,7 +203,7 @@ def orc():
 
 
 def ref():
-    """The compiled reference, or None when it was never built (needs /root/reference once)."""
+    """The compiled reference, or None when it was never built."""
     global _ref
     if _ref is None:
         so = os.path.join(ROOT, "oracle", "_ref", "libhts_ref.so")
@@ -53,6 +230,7 @@ def orc_rans_nx16_decode(data, out_size):
     return bytes(out[: n.value])
 
 
+@stored_reference(digest=True)
 def ref_rans_nx16_decode(data, out_size):
     r = ref()
     out = (C.c_uint8 * max(1, out_size))()
@@ -63,6 +241,7 @@ def ref_rans_nx16_decode(data, out_size):
     return bytes(out[: n.value])
 
 
+@stored_reference
 def ref_rans_nx16_encode(data, order):
     r = ref()
     cap = r.rans_compress_bound_4x16(C.c_uint(len(data)), C.c_int(order))
@@ -71,6 +250,50 @@ def ref_rans_nx16_encode(data, order):
     p = r.rans_compress_to_4x16(buf(data), C.c_uint(len(data)), out, C.byref(n), C.c_int(order))
     assert p, "reference encoder failed"
     return bytes(out[: n.value])
+
+
+@stored_reference(digest=True)
+def ref_rans_nx16_decode_scalar(data, out_size):
+    """ref_rans_nx16_decode through the reference's scalar decoders (rans_set_cpu(0), rANS_static4x16pr.c:1191):
+    its SIMD decoders read differently once a damaged stream runs dry."""
+    r = ref()
+    r.rans_set_cpu(0)
+    try:
+        return ref_rans_nx16_decode.__wrapped__(data, out_size)
+    finally:
+        r.rans_set_cpu(-1)
+
+
+@stored_reference(digest=True)
+def ref_rans_nx16_encoded(data, order):
+    """ref_rans_nx16_encode as a Digest (length, first bytes, hash): for tests that only compare with it."""
+    return ref_rans_nx16_encode.__wrapped__(data, order)
+
+
+@stored_reference(digest=True)
+def ref_rans_4x8_encoded(data, order):
+    """ref_rans_4x8(data, order) as a Digest."""
+    return ref_rans_4x8.__wrapped__(data, order)
+
+
+@stored_reference(digest=True)
+def ref_arith_encoded(data, order):
+    """ref_arith(data, order) as a Digest."""
+    return ref_arith.__wrapped__(data, order)
+
+
+@stored_reference(digest=True)
+def ref_fqz_compressed(quals, lens, flags=None, strat=0, vers=4):
+    """ref_fqz_compress as a Digest."""
+    return ref_fqz_compress.__wrapped__(quals, lens, flags, strat, vers)
+
+
+@stored_reference
+def ref_arith_compress_bounds(pairs):
+    """arith_compress_bound(size, order) for every (size, order) pair."""
+    r = ref()
+    r.arith_compress_bound.restype = C.c_uint
+    return [r.arith_compress_bound(C.c_uint(s), C.c_int(o)) for s, o in pairs]
 
 
 def golden_raw(name):
@@ -143,6 +366,7 @@ def orc_bgzf_scan(data):
     return n, [(off[i], ln[i]) for i in range(n)]
 
 
+@stored_reference(digest=True)
 def ref_bgzf_read_all(data, threads=0):
     """Decompress a whole BGZF file image with the compiled reference: hopen("mem:") ->
     bgzf_hopen -> [bgzf_mt] -> bgzf_read loop.  Returns (bytes, errcode)."""
@@ -217,6 +441,7 @@ def bam_header(n_ref=1, name=b"chr1", length=250000000):
         struct.pack("<i", len(name) + 1) + name + b"\0" + struct.pack("<i", length)
 
 
+@stored_reference(digest=True, limit=400000)
 def ref_bam_read_all(img):
     """Every record of a BGZF BAM image through the compiled reference's bam_hdr_read + bam_read1.
     Returns list of (core tuple, data bytes, return code)."""
@@ -259,6 +484,7 @@ class KString(C.Structure):       # kstring_t, htslib/kstring.h
     _fields_ = [("l", C.c_size_t), ("m", C.c_size_t), ("s", C.c_void_p)]
 
 
+@stored_reference(digest=True, limit=200000)
 def ref_sam_format_all(img):
     """Every record of a BGZF BAM image through the compiled reference's bam_read1 + sam_format1.
     Returns (target names, [line bytes or None when sam_format1 fails])."""
@@ -334,6 +560,7 @@ def orc_rans_4x8_decode(data, cap):
     return None if rc else bytes(out[: n.value])
 
 
+@stored_reference(digest=lambda kw: "comp" in kw)
 def ref_rans_4x8(data=None, order=None, comp=None):
     """reference rans_compress / rans_uncompress (rANS_static.c:829-850)."""
     r = ref()
@@ -351,6 +578,7 @@ def ref_rans_4x8(data=None, order=None, comp=None):
     return res
 
 
+@stored_reference(digest=lambda kw: "comp" in kw)
 def ref_arith(data=None, order=None, comp=None, cap=None):
     """reference arith_compress_to / arith_uncompress_to (arith_dynamic.c:730, :1033)."""
     r = ref()
@@ -367,6 +595,7 @@ def ref_arith(data=None, order=None, comp=None, cap=None):
     return bytes(out[: n.value]) if p else None
 
 
+@stored_reference(limit=40000)
 def ref_tok3_encode(names, level=3, use_arith=0):
     """reference tok3_encode_names (tokenise_name3.c:1456): names is the NUL- or LF-separated blob."""
     r = ref()
@@ -380,6 +609,7 @@ def ref_tok3_encode(names, level=3, use_arith=0):
     return res
 
 
+@stored_reference(digest=True)
 def ref_tok3_decode(comp):
     r = ref()
     r.tok3_decode_names.restype = C.c_void_p
@@ -392,12 +622,17 @@ def ref_tok3_decode(comp):
     return res
 
 
+@C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_uint, C.c_void_p, C.POINTER(C.c_uint))
+def _orc_arith_uncompress_to(inp, in_size, out, out_size):
+    """arith_uncompress_to's contract (out, or NULL on error) over the oracle's own decoder."""
+    return out if orc().orc_arith_decode(C.c_void_p(inp), C.c_uint32(in_size), C.c_void_p(out), out_size) == 0 else None
+
+
 def orc_tok3_decode(comp):
-    """oracle tok3 decode; the adaptive arithmetic sub-coder is oracle/_ref's arith_uncompress_to."""
+    """oracle tok3 decode; the adaptive arithmetic sub-coder is the oracle's (orc_arith_decode)."""
     o = orc()
     o.orc_tok3_decode.restype = C.c_void_p
-    r = ref()
-    fn = C.cast(r.arith_uncompress_to, C.c_void_p) if r is not None else C.c_void_p(0)
+    fn = C.cast(_orc_arith_uncompress_to, C.c_void_p)
     n = C.c_uint32(0)
     p = o.orc_tok3_decode(buf(comp), C.c_uint32(len(comp)), C.byref(n), fn)
     if not p:
@@ -411,6 +646,7 @@ class FqzSlice(C.Structure):      # fqz_slice, htscodecs/htscodecs/fqzcomp_qual.
     _fields_ = [("num_records", C.c_int), ("len", C.POINTER(C.c_uint32)), ("flags", C.POINTER(C.c_uint32))]
 
 
+@stored_reference
 def ref_fqz_compress(quals, lens, flags=None, strat=0, vers=4):
     """reference fqz_compress (fqzcomp_qual.c:1615): quals = concatenated quality bytes, lens = record lengths."""
     r = ref()
@@ -427,6 +663,7 @@ def ref_fqz_compress(quals, lens, flags=None, strat=0, vers=4):
     return res
 
 
+@stored_reference(digest=True)
 def ref_fqz_decompress(comp):
     r = ref()
     r.fqz_decompress.restype = C.c_void_p
@@ -463,6 +700,7 @@ def orc_arith_decode(comp, cap):
     return None if rc != 0 else bytes(out[: n.value])
 
 
+@stored_reference(digest=True, limit=200000)
 def ref_cram_read_all(path, fasta=None, decode_md=0):
     """Every record of a CRAM file through the compiled reference: hts_open + sam_hdr_read + sam_read1 (-> cram_get_bam_seq).
     Returns list of (core tuple, data bytes)."""
@@ -501,6 +739,24 @@ def ref_cram_read_all(path, fasta=None, decode_md=0):
 
 def ref_write_cram(sam_path, fasta, out_path, version="3.0", int_opts=()):
     """SAM -> CRAM through the compiled reference (hts_open "wc", sam_write1).  int_opts: (hts_fmt_option, int) pairs."""
+    n, img = _ref_write_cram(sam_path, fasta, version, [list(o) for o in int_opts])
+    with open(out_path, "wb") as f:
+        f.write(img)
+    return n
+
+
+@stored_reference(limit=100000)
+def _ref_write_cram(sam_path, fasta, version, int_opts):
+    """(records written, file image) of ref_write_cram."""
+    import tempfile
+    with tempfile.TemporaryDirectory() as td:
+        out_path = os.path.join(td, "out.cram")
+        n = _ref_write_cram_to(sam_path, fasta, out_path, version, int_opts)
+        with open(out_path, "rb") as f:
+            return n, f.read()
+
+
+def _ref_write_cram_to(sam_path, fasta, out_path, version, int_opts):
     r = ref()
     r.hts_open.restype = C.c_void_p
     r.hts_open.argtypes = [C.c_char_p, C.c_char_p]
@@ -538,6 +794,7 @@ def ref_write_cram(sam_path, fasta, out_path, version="3.0", int_opts=()):
     return n
 
 
+@stored_reference(digest=True, limit=200000)
 def ref_cram_sam_text(path, fasta=None, decode_md=0):
     """SAM text of a CRAM file through the compiled reference: sam_read1 + sam_format1.  Returns (target names, [line bytes])."""
     r = ref()
@@ -580,6 +837,7 @@ def ref_cram_sam_text(path, fasta=None, decode_md=0):
     return names, lines
 
 
+@stored_reference(limit=20000)
 def ref_read_sam_records(path):
     """(header text, [(core tuple, data bytes)]) of a SAM / BAM / CRAM file through the compiled reference (sam_hdr_read, sam_read1)."""
     r = ref()

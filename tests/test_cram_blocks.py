@@ -25,8 +25,7 @@ def test_scan_matches_expected_structure():
         comp = img[int(b["data_off"]):int(b["data_off"]) + int(b["comp_size"])].tobytes()
         out = orc_rans_nx16_decode(comp, int(b["uncomp_size"]))
         assert out is not None and len(out) == int(b["uncomp_size"])
-        if ref() is not None:
-            assert ref_rans_nx16_decode(comp, int(b["uncomp_size"])) == out
+        assert ref_rans_nx16_decode(comp, int(b["uncomp_size"])) == out
     bad = img.copy(); bad[0] = ord("X")
     with pytest.raises(H.HgpuError):
         H.cram_scan_blocks(bad)
@@ -61,9 +60,15 @@ def _expect(img, b):
     if m == 1: return __import__("zlib").decompress(comp, 31)
     if m == 4: return L.orc_rans_4x8_decode(comp, us)
     if m == 5: return L.orc_rans_nx16_decode(comp, us)
-    if m == 6: return L.ref_arith(comp=comp, cap=us) if L.ref() is not None else None
-    if m == 7: return L.ref_fqz_decompress(comp) if L.ref() is not None else None
-    if m == 8: return L.orc_tok3_decode(comp) if (comp[8] == 0 or L.ref() is not None) else None
+    if m == 6:
+        out = L.orc_arith_decode(comp, us)
+        assert out == L.ref_arith(comp=comp, cap=us)
+        return out
+    if m == 7:
+        out = L.orc_fqz_decode(comp)
+        assert out == L.ref_fqz_decompress(comp)
+        return out
+    if m == 8: return L.orc_tok3_decode(comp)
     return None
 
 
@@ -89,8 +94,8 @@ def test_uncompress_all_blocks_in_one_call(name):
             seen[m] += 1
     if name.endswith("v31.cram"): assert seen[5] == 14 and seen[8] == 1
     if name.endswith("v30.cram"): assert seen[4] == 9
-    if name.endswith("arith.cram") and ref() is not None: assert seen[6] == 30 and seen[8] == 4
-    if name.endswith("fqz.cram") and ref() is not None: assert seen[7] == 1
+    if name.endswith("arith.cram"): assert seen[6] == 30 and seen[8] == 4
+    if name.endswith("fqz.cram"): assert seen[7] == 1
     # one flipped payload bit: that block fails its CRC (cram_io.c:1585-1592), every other block is unaffected
     victim = int(np.argmax(blocks["comp_size"]))
     bad = img.copy(); bad[int(blocks[victim]["data_off"]) + 5] ^= 0x10
@@ -117,7 +122,7 @@ def test_scan_foreign_writer_files(name):
         assert zlib.crc32(img[o - hl:o + cs].tobytes()) == int.from_bytes(img[o + cs:o + cs + 4].tobytes(), "little")
         want = _expect(img, b)
         assert want is not None and len(want) == us, (int(b["method"]), cs, us)
-        if int(b["method"]) == 4 and us and L.ref() is not None:         # the oracle agrees with the reference on foreign rANS streams
+        if int(b["method"]) == 4 and us:         # the oracle agrees with the reference on foreign rANS streams
             assert L.ref_rans_4x8(comp=comp) == want
 
 

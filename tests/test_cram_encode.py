@@ -94,7 +94,6 @@ def roundtrip(tmp_path, entry_ctx, sam, rps, minor, with_ref=False):
     return 0, img
 
 
-@pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
 @pytest.mark.parametrize("rps,minor,with_ref", [(0, 0, False), (3, 1, False), (0, 1, True), (2, 0, True)])
 @pytest.mark.parametrize("sam", SAMS)
 def test_hostsim_reference_reads_back_what_we_wrote(tmp_path, sam, rps, minor, with_ref):
@@ -116,7 +115,7 @@ def test_hostsim_reference_reads_back_what_we_wrote(tmp_path, sam, rps, minor, w
         assert tuple(int(got["core"][i][f]) for f in NAMES) == wc and got["data"][i] == wd, (sam, i)
 
 
-@pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
+@pytest.mark.skipif(ref() is None, reason="the 10 000 synthetic records come from the reference's SAM reader; oracle/_ref not built")
 def test_hostsim_synthetic_10000_reads(tmp_path):
     sam = str(tmp_path / "syn.sam")
     n = T._synthetic_sam(sam, n=10000, seed=21)
@@ -139,7 +138,6 @@ def test_hostsim_synthetic_10000_reads(tmp_path):
 
 
 @pytest.mark.gpu
-@pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
 @pytest.mark.parametrize("minor", [0, 1])
 def test_gpu_reference_reads_back_what_we_wrote(tmp_path, minor):
     ctx = H.Context(0)
@@ -150,6 +148,9 @@ def test_gpu_reference_reads_back_what_we_wrote(tmp_path, minor):
             assert rc in (0, -6), (sam, rc, img)
             done += rc == 0
     assert done >= 60
+    if ref() is None:                                       # the 10 000 synthetic records come from the reference's SAM reader
+        ctx.close()
+        return
     # a 10 000-read slice: compressed by the device codecs, smaller than the records, read back by the reference
     sam = str(tmp_path / "syn.sam")
     n = T._synthetic_sam(sam, n=10000, seed=21)

@@ -21,7 +21,9 @@ class KS(C.Structure):
     _fields_ = [("l", C.c_size_t), ("m", C.c_size_t), ("s", C.c_char_p)]
 
 
-def _reference_descriptions(path):
+@L.stored_reference(limit=60000)
+def ref_cram_descriptions(path):
+    """cram_describe_encodings of every container's compression header."""
     r = L.ref()
     r.cram_open.restype = C.c_void_p; r.cram_open.argtypes = [C.c_char_p, C.c_char_p]
     r.cram_close.argtypes = [C.c_void_p]
@@ -54,11 +56,10 @@ def _reference_descriptions(path):
     return out
 
 
-@pytest.mark.skipif(L.ref() is None, reason="needs oracle/_ref")
 @pytest.mark.parametrize("name", FILES)
 def test_description_equals_reference(name):
     path = os.path.join(L.GOLD, "htslib", name)
-    want = _reference_descriptions(path)
+    want = ref_cram_descriptions(path)
     img = np.fromfile(path, dtype=np.uint8)
     blocks, ver = H.cram_scan_blocks(img)
     got = []
@@ -96,7 +97,6 @@ def test_rejects_garbage():
             pass
 
 
-@pytest.mark.skipif(L.ref() is None, reason="needs oracle/_ref")
 @pytest.mark.parametrize("name", FILES)
 def test_containers_and_slices_equal_reference(name):
     """Every container header field the reference exposes (htslib/cram.h:190-216) and every slice header field
@@ -112,6 +112,41 @@ def test_containers_and_slices_equal_reference(name):
         if len(mine):
             assert int(np.where(blocks["container"] == i)[0][0]) == int(c["first_block"])
             assert int(mine[0]["data_off"]) - int(mine[0]["hdr_len"]) == int(c["data_off"])
+    slices = 0
+    ci, bi = 1, int(cont[0]["n_blocks"])
+    for length, n_blocks, n_records, bases, landmarks, coords, slice_hdrs in ref_cram_containers(path):
+        m = cont[ci]
+        assert length == int(m["length"])
+        assert n_blocks == int(m["n_blocks"])
+        assert n_records == int(m["n_records"])
+        assert bases == int(m["bases"])
+        assert len(landmarks) == int(m["n_landmarks"])
+        assert landmarks == lm[int(m["landmark0"]):int(m["landmark0"]) + len(landmarks)].tolist()
+        assert coords == (int(m["ref_id"]), int(m["start"]), int(m["span"]))
+        for k in range(int(m["n_blocks"])):
+            if k in slice_hdrs:
+                h_blocks, h_embed, h_coords = slice_hdrs[k]
+                x = blocks[bi]
+                comp = img[int(x["data_off"]):int(x["data_off"]) + int(x["comp_size"])].tobytes()
+                payload = comp if int(x["method"]) == 0 else zlib.decompress(comp, 31)
+                s, ids = H.cram_parse_slice_header(payload, ver[0])
+                assert h_blocks == int(s["n_blocks"])
+                assert h_embed == int(s["ref_base_id"])
+                assert h_coords == (int(s["ref_id"]), int(s["start"]), int(s["span"]))
+                # the slice's external blocks carry exactly the content ids its header lists
+                follow = blocks[bi + 1: bi + 1 + int(s["n_blocks"])]
+                ext = follow[follow["content_type"] == 4]                  # the CORE block (type 5, id 0) is not listed
+                assert sorted(int(v) for v in ext["content_id"]) == sorted(ids)
+                slices += 1
+            bi += 1
+        ci += 1
+    assert ci == len(cont) and slices >= 1
+
+
+@L.stored_reference
+def ref_cram_containers(path):
+    """Per data container: (length, blocks, records, bases, landmarks, (ref id, start, span), {block index of a
+    mapped slice header: (blocks, embedded reference id, (ref id, start, span))}) through the reference's accessors."""
     r = L.ref()
     r.cram_open.restype = C.c_void_p; r.cram_open.argtypes = [C.c_char_p, C.c_char_p]
     r.cram_close.argtypes = [C.c_void_p]
@@ -129,45 +164,27 @@ def test_containers_and_slices_equal_reference(name):
     r.cram_slice_hdr_get_embed_ref_id.argtypes = [C.c_void_p]
     r.cram_slice_hdr_get_coords.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     fd = r.cram_open(path.encode(), b"r")                             # consumes container 0, the SAM header container
-    ci, bi = 1, int(cont[0]["n_blocks"])
-    slices = 0
+    out = []
     while True:
         c = r.cram_read_container(fd)
         if not c:
             break
-        m = cont[ci]
-        assert r.cram_container_get_length(c) == int(m["length"])
-        assert r.cram_container_get_num_blocks(c) == int(m["n_blocks"])
-        assert r.cram_container_get_num_records(c) == int(m["n_records"])
-        assert r.cram_container_get_num_bases(c) == int(m["bases"])
         nl = C.c_int32(0)
         lp = r.cram_container_get_landmarks(c, C.byref(nl))
-        assert nl.value == int(m["n_landmarks"])
-        assert [lp[k] for k in range(nl.value)] == lm[int(m["landmark0"]):int(m["landmark0"]) + nl.value].tolist()
         rid, st, sp = C.c_int(0), C.c_int64(0), C.c_int64(0)
         r.cram_container_get_coords(c, C.byref(rid), C.byref(st), C.byref(sp))
-        assert (rid.value, st.value, sp.value) == (int(m["ref_id"]), int(m["start"]), int(m["span"]))
-        for k in range(int(m["n_blocks"])):
+        nb = r.cram_container_get_num_blocks(c)
+        cont = [r.cram_container_get_length(c), nb, r.cram_container_get_num_records(c), r.cram_container_get_num_bases(c),
+                [lp[k] for k in range(nl.value)], (rid.value, st.value, sp.value), {}]
+        for k in range(nb):
             b = r.cram_read_block(fd)
             assert b
             if r.cram_block_get_content_type(b) == 2:                     # MAPPED_SLICE header
                 assert r.cram_uncompress_block(b) == 0
                 h = r.cram_decode_slice_header(fd, b)
                 assert h
-                x = blocks[bi]
-                comp = img[int(x["data_off"]):int(x["data_off"]) + int(x["comp_size"])].tobytes()
-                payload = comp if int(x["method"]) == 0 else zlib.decompress(comp, 31)
-                s, ids = H.cram_parse_slice_header(payload, ver[0])
-                assert r.cram_slice_hdr_get_num_blocks(h) == int(s["n_blocks"])
-                assert r.cram_slice_hdr_get_embed_ref_id(h) == int(s["ref_base_id"])
                 r.cram_slice_hdr_get_coords(h, C.byref(rid), C.byref(st), C.byref(sp))
-                assert (rid.value, st.value, sp.value) == (int(s["ref_id"]), int(s["start"]), int(s["span"]))
-                # the slice's external blocks carry exactly the content ids its header lists
-                follow = blocks[bi + 1: bi + 1 + int(s["n_blocks"])]
-                ext = follow[follow["content_type"] == 4]                  # the CORE block (type 5, id 0) is not listed
-                assert sorted(int(v) for v in ext["content_id"]) == sorted(ids)
-                slices += 1
-            bi += 1
-        ci += 1
+                cont[6][k] = (r.cram_slice_hdr_get_num_blocks(h), r.cram_slice_hdr_get_embed_ref_id(h), (rid.value, st.value, sp.value))
+        out.append(tuple(cont))
     r.cram_close(fd)
-    assert ci == len(cont) and slices >= 1
+    return out

@@ -6,7 +6,7 @@ tests/test_oracle_arith.py."""
 import glob, os, random
 import pytest
 import htslib_b200 as H
-from _libs import GOLD, golden_raw, ref, ref_arith
+from _libs import GOLD, golden_raw, ref, ref_arith, sampled
 from test_oracle_rans import _synth
 
 pytestmark = pytest.mark.gpu
@@ -34,7 +34,6 @@ def test_golden_streams(ctx):
         assert data == w, nm
 
 
-@pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
 def test_seeded_all_orders_and_corrupt(ctx):
     rng = random.Random(77)
     comps, wants = [], []
@@ -42,11 +41,12 @@ def test_seeded_all_orders_and_corrupt(ctx):
         for kind in ("q4", "q40", "runs", "one", "u32", "rand"):
             for n in (1, 3, 32, 100, 1000, 4099, 30001):
                 raw = _synth(rng, n, kind)
-                comps.append(ref_arith(raw, order)); wants.append(raw)
+                with sampled():
+                    comps.append(ref_arith(raw, order)); wants.append(raw)
     res = ctx.arith_decode(comps, [len(w) for w in wants])
     for i, ((st, data), w) in enumerate(zip(res, wants)):
         assert st == 0 and data == w, (i, comps[i][:4].hex(), len(w))
-    base = ref_arith(_synth(rng, 5000, "q40"), 65)
+    base = ref_arith(_synth(rng, 5000, "q40"), 65, store_always=True)
     bad = []
     for _ in range(50):
         c = bytearray(base); k = rng.randrange(8, len(c)); c[k] ^= 1 << rng.randrange(8); bad.append(bytes(c))

@@ -6,7 +6,7 @@ import os, sys, tempfile, zlib
 import numpy as np
 import pytest
 import htslib_b200 as H
-from _libs import ROOT, GOLD, Bam1, BamCore, bam_header, bam_header_len, bgzf_file, orc, orc_bam_unpack_all, orc_bgzf_scan, ref, buf
+from _libs import ROOT, GOLD, Bam1, BamCore, bam_header, bam_header_len, bgzf_file, orc, orc_bam_unpack_all, orc_bgzf_scan, ref, buf, stored_reference
 sys.path.insert(0, ROOT)
 from tools import synth
 
@@ -23,17 +23,10 @@ def orc_pack(recs):
     return bytes(out)
 
 
-@pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
-def test_oracle_pack_matches_reference_bam_write1():
-    """reference: bam_read1 every record of a fixture, bam_write1 it to an uncompressed ('wu') BGZF
-    file; the file body after the header must equal the oracle's packing of the oracle's unpacking."""
+@stored_reference(digest=True)
+def ref_bam_write1_all(path):
+    """bam_read1 every record of a BAM file and bam_write1 it to an uncompressed ('wu') BGZF file: that file."""
     r = ref()
-    path = os.path.join(GOLD, "htslib", "range.bam")
-    img = open(path, "rb").read()
-    _, blocks = orc_bgzf_scan(img)
-    stream = b"".join(zlib.decompress(img[o + 18:o + l - 8], -15) for o, l in blocks)
-    h = bam_header_len(stream)
-    recs, _ = orc_bam_unpack_all(stream[h:])
     r.bgzf_open.restype = C.c_void_p; r.bgzf_open.argtypes = [C.c_char_p, C.c_char_p]
     r.bgzf_close.argtypes = [C.c_void_p]
     r.bam_hdr_read.restype = C.c_void_p; r.bam_hdr_read.argtypes = [C.c_void_p]
@@ -50,7 +43,19 @@ def test_oracle_pack_matches_reference_bam_write1():
         while r.bam_read1(fin, b) >= 0:
             assert r.bam_write1(fout, b) > 0
         r.bam_destroy1(b); r.sam_hdr_destroy(hdr); r.bgzf_close(fin); r.bgzf_close(fout)
-        want = open(outp, "rb").read()
+        return open(outp, "rb").read()
+
+
+def test_oracle_pack_matches_reference_bam_write1():
+    """reference: bam_read1 every record of a fixture, bam_write1 it to an uncompressed ('wu') BGZF
+    file; the file body after the header must equal the oracle's packing of the oracle's unpacking."""
+    path = os.path.join(GOLD, "htslib", "range.bam")
+    img = open(path, "rb").read()
+    _, blocks = orc_bgzf_scan(img)
+    stream = b"".join(zlib.decompress(img[o + 18:o + l - 8], -15) for o, l in blocks)
+    h = bam_header_len(stream)
+    recs, _ = orc_bam_unpack_all(stream[h:])
+    want = ref_bam_write1_all(path)
     assert orc_pack(recs) == want
     assert want == stream[h:]            # a read/write round trip reproduces the record stream
 

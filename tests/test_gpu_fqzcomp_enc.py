@@ -33,15 +33,14 @@ def test_round_trip_through_reference_and_own_decoder():
         comps = []
         for (q, lens), (st, comp) in zip(blocks, res):
             assert st == 0, (strat, len(q))
-            if L.ref() is not None:
-                assert L.ref_fqz_decompress(comp) == q, (strat, len(q))
+            assert L.ref_fqz_decompress(comp) == q, (strat, len(q))
             comps.append(comp)
         back = H.fqz_decode(ctx, comps, [len(b[0]) for b in blocks])
         for (q, _), (st, data) in zip(blocks, back):
             assert st == 0 and data == q
-        if strat == 0 and L.ref() is not None:                         # size against the reference encoder, same strategy
+        if strat == 0:                         # size against the reference encoder, same strategy
             ours = sum(len(c) for c in comps[-4:])
-            theirs = sum(len(L.ref_fqz_compress(q, lens, None, 0)) for q, lens in blocks[-4:])
+            theirs = sum(len(L.ref_fqz_compressed(q, lens, None, 0)) for q, lens in blocks[-4:])
             assert ours < 1.1 * theirs, (ours, theirs)
     # rejected: lengths that do not tile the block
     (st, _), = H.fqz_encode(ctx, [b"\x05" * 100], [[60, 30]])

@@ -5,7 +5,7 @@ import glob, os, random
 import numpy as np
 import pytest
 import htslib_b200 as H
-from _libs import GOLD, golden_raw, orc_rans_4x8_decode, ref, ref_rans_4x8
+from _libs import GOLD, golden_raw, orc_rans_4x8_decode, ref, ref_rans_4x8, sampled
 from test_oracle_rans import _synth
 
 pytestmark = pytest.mark.gpu
@@ -32,7 +32,6 @@ def test_golden_and_cram30_blocks(ctx):
         assert st == 0 and data == w
 
 
-@pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
 def test_seeded_and_corrupt(ctx):
     rng = random.Random(12)
     comps, wants = [], []
@@ -40,12 +39,13 @@ def test_seeded_and_corrupt(ctx):
         for kind in ("q4", "q40", "runs", "one", "u32", "rand"):
             for n in (1, 3, 4, 5, 31, 100, 1000, 4099, 70001):
                 raw = _synth(rng, n, kind)
-                comps.append(ref_rans_4x8(raw, order)); wants.append(raw)
+                with sampled():
+                    comps.append(ref_rans_4x8(raw, order)); wants.append(raw)
     res = ctx.rans4x8_decode(comps, [len(w) for w in wants])
     for i, ((st, data), w) in enumerate(zip(res, wants)):
         assert st == 0 and data == w, i
     # damaged payload bytes: same bytes or same failure as the oracle
-    base = ref_rans_4x8(_synth(rng, 6000, "q40"), 1)
+    base = ref_rans_4x8(_synth(rng, 6000, "q40"), 1, store_always=True)
     bad = []
     for _ in range(60):
         c = bytearray(base); k = rng.randrange(len(c) // 2, len(c)); c[k] ^= 1 << rng.randrange(8); bad.append(bytes(c))

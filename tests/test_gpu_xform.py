@@ -6,9 +6,9 @@ import random
 import numpy as np
 import pytest
 import htslib_b200 as H
-from _libs import ref
+from _libs import ref, stored_reference
 
-pytestmark = [pytest.mark.gpu, pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")]
+pytestmark = [pytest.mark.gpu]
 u8p = C.POINTER(C.c_uint8)
 
 
@@ -58,35 +58,66 @@ def rle_dec(L, lit, run, syms, cap):
     return bytes(out[:ol.value]) if p else None
 
 
+@stored_reference(digest=True)
+def ref_xform_pack(data):
+    return pack(bind(ref()), data)
+
+
+@stored_reference
+def ref_xform_unpack_meta(meta, n):
+    """(bytes of meta used, symbol count, map) from the reference's hts_unpack_meta."""
+    R = bind(ref())
+    mp = (C.c_uint8 * 16)(); ns = C.c_int(-1)
+    used = R.hts_unpack_meta((C.c_uint8 * len(meta)).from_buffer_copy(meta), len(meta), n, mp, C.byref(ns))
+    return used, ns.value, bytes(mp)
+
+
+@stored_reference
+def ref_xform_unpack_refused(packed, n, ns, mp):
+    R = bind(ref())
+    out = (C.c_uint8 * max(1, n))()
+    pb = (C.c_uint8 * max(1, len(packed))).from_buffer_copy(packed or b"\0")
+    return not R.hts_unpack(pb, len(packed), out, n, ns, (C.c_uint8 * 16).from_buffer_copy(mp))
+
+
+@stored_reference(digest=True)
+def ref_xform_rle_encode(data, syms):
+    return rle_enc(bind(ref()), data, syms)
+
+
+@stored_reference(digest=True)
+def ref_xform_rle_decode(lit, run, syms, cap):
+    return rle_dec(bind(ref()), lit, run, syms, cap)
+
+
 def test_pack_unpack_equal_the_reference():
-    G, R = bind(H.lib()), bind(ref())
+    G = bind(H.lib())
     rng = random.Random(12)
     for nsym in (1, 2, 3, 4, 5, 16, 17, 40):
         alphabet = rng.sample(range(256), nsym)
         for n in (0, 1, 2, 3, 7, 8, 9, 15, 16, 17, 1000, 70001):
             data = bytes(rng.choice(alphabet) for _ in range(n))
-            want = pack(R, data); got = pack(G, data)
+            want = ref_xform_pack(data); got = pack(G, data)
             assert got == want, (nsym, n)
             if want is None:
                 continue
-            meta, packed = want
+            meta, packed = got
             # meta -> map, then unpack on the device == the input
             mp = (C.c_uint8 * 16)(); ns = C.c_int(-1)
             mb = (C.c_uint8 * len(meta)).from_buffer_copy(meta)
             used = G.hts_unpack_meta(mb, len(meta), n, mp, C.byref(ns))
-            mp2 = (C.c_uint8 * 16)(); ns2 = C.c_int(-1)
-            assert used == R.hts_unpack_meta(mb, len(meta), n, mp2, C.byref(ns2)) and ns.value == ns2.value and bytes(mp) == bytes(mp2)
+            assert (used, ns.value, bytes(mp)) == ref_xform_unpack_meta(meta, n)
             out = (C.c_uint8 * max(1, n))()
             pb = (C.c_uint8 * max(1, len(packed))).from_buffer_copy(packed or b"\0")
             assert G.hts_unpack(pb, len(packed), out, n, ns.value, mp)
             assert bytes(out[:n]) == data
             if n > 8 and ns.value > 1:                                   # too little packed data for the claimed output: refused, as the reference does
                 assert not G.hts_unpack(pb, max(0, len(packed) - 2), out, n, ns.value, mp)
-                assert not R.hts_unpack(pb, max(0, len(packed) - 2), out, n, ns.value, mp)
+                assert ref_xform_unpack_refused(packed[:max(0, len(packed) - 2)], n, ns.value, bytes(mp))
 
 
 def test_rle_equal_the_reference():
-    G, R = bind(H.lib()), bind(ref())
+    G = bind(H.lib())
     rng = random.Random(13)
     cases = [b"", b"a", b"aa", b"ab", b"a" * 31, b"a" * 32, b"a" * 33, b"a" * 64 + b"b", b"ab" * 100, b"a" * 100000]
     for n in (50, 257, 5000, 70000):
@@ -96,12 +127,12 @@ def test_rle_equal_the_reference():
         cases.append(b"".join(runs)[:n])
     for data in cases:
         for syms in (None, [ord("A"), ord("#")]):
-            want = rle_enc(R, data, syms); got = rle_enc(G, data, syms)
+            want = ref_xform_rle_encode(data, syms); got = rle_enc(G, data, syms)
             assert got == want, (len(data), syms)
-            lit, run, ss = want
-            assert rle_dec(G, lit, run, ss, len(data)) == data == (rle_dec(R, lit, run, ss, len(data)) if data else data)
+            lit, run, ss = got
+            assert rle_dec(G, lit, run, ss, len(data)) == data == (ref_xform_rle_decode(lit, run, ss, len(data)) if data else data)
             if len(data) > 40 and lit != data:                           # an output buffer that is too small: refused
-                assert rle_dec(G, lit, run, ss, len(data) - 1) is None and rle_dec(R, lit, run, ss, len(data) - 1) is None
+                assert rle_dec(G, lit, run, ss, len(data) - 1) is None and ref_xform_rle_decode(lit, run, ss, len(data) - 1) is None
 
 
 def test_version_string():

@@ -9,7 +9,7 @@ import subprocess
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-B = os.path.join(ROOT, "integration", "_build")
+B = os.path.join(ROOT, "oracle", "_ref", "integration")
 G = os.path.join(ROOT, "tests", "golden", "htslib")
 have = os.path.exists(os.path.join(B, "test_view")) and os.path.exists(os.path.join(B, "stock", "test_view"))
 
@@ -40,7 +40,7 @@ def test_integration_build_links_the_gpu_symbols():
 
 
 gpu = pytest.mark.gpu
-need = pytest.mark.skipif(not have, reason="integration/_build not built")
+need = pytest.mark.skipif(not have, reason="oracle/_ref/integration not built (needs the reference sources)")
 
 
 @gpu

@@ -36,13 +36,11 @@ def check_against_reference(img):
     return len(recs)
 
 
-@pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
 @pytest.mark.parametrize("path", BAMS, ids=os.path.basename)
 def test_fixture_bams(path):
     check_against_reference(open(path, "rb").read())
 
 
-@pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
 def test_synthetic_records_and_odd_cases():
     stream, offs = synth.bam_records(3, 3000)
     rng = random.Random(4)
@@ -66,7 +64,6 @@ def test_synthetic_records_and_odd_cases():
     check_against_reference(bgzf_file(bam_header() + stream[:offs[200]], 1, block=777))
 
 
-@pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
 def test_invalid_records_rejected_like_reference():
     stream, offs = synth.bam_records(5, 20)
     good = bytearray(stream[:offs[5]])

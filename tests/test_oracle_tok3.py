@@ -11,10 +11,6 @@ import _libs as L
 TOK3 = sorted(glob.glob(os.path.join(L.GOLD, "htscodecs", "names", "tok3", "*")))
 
 
-def _is_arith(comp):
-    return comp[8] != 0
-
-
 def _plain(path):
     base = os.path.basename(path).rsplit(".", 1)[0]            # 01.names.3 -> 01.names
     return open(os.path.join(L.GOLD, "htscodecs", "names", base), "rb").read().replace(b"\n", b"\0")
@@ -23,8 +19,6 @@ def _plain(path):
 @pytest.mark.parametrize("path", TOK3, ids=[os.path.basename(p) for p in TOK3])
 def test_golden(path):
     comp = open(path, "rb").read()
-    if _is_arith(comp) and L.ref() is None:
-        pytest.skip("arith sub-coder needs oracle/_ref")
     got = L.orc_tok3_decode(comp)
     assert got is not None
     assert got == _plain(path)
@@ -46,7 +40,6 @@ def _names(rng, n, style):
     return ("\0".join(out) + "\0").encode()
 
 
-@pytest.mark.skipif(L.ref() is None, reason="needs oracle/_ref")
 @pytest.mark.parametrize("style", [0, 1, 2])
 @pytest.mark.parametrize("level,arith", [(1, 0), (3, 0), (7, 0), (9, 0), (1, 1), (3, 1)])  # level >= 5 with arith wants bzip2 (X_EXT), not compiled into oracle/_ref
 def test_vs_reference_seeded(style, level, arith):
@@ -58,7 +51,6 @@ def test_vs_reference_seeded(style, level, arith):
     assert L.orc_tok3_decode(comp) == want
 
 
-@pytest.mark.skipif(L.ref() is None, reason="needs oracle/_ref")
 def test_corrupt_agrees_with_reference():
     rng = random.Random(7)
     blob = _names(rng, 200, 0)

@@ -45,6 +45,7 @@ def scan_containers(H, img):
 def run(ctx, reads=100000, tiles=20, cpu=True, decode_md=0):
     import htslib_b200 as H
     from _libs import ref, ref_write_cram, ref_cram_read_all
+    ref_cram_read_all = ref_cram_read_all.__wrapped__              # the live reference: the checks below slice its records
     import test_cram_records as T
     if ref() is None:
         return {"error": "oracle/_ref not built"}

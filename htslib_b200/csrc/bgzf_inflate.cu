@@ -15,8 +15,8 @@
 //     [31:16] value (literal / length base / distance base / sub-table offset)
 //     [15:8]  extra-bit count (or sub-table index bits)
 //     [7:4]   kind   [3:0] code bits consumed
-// The CRC-32 of the output is computed by the same warp: 32 equal chunks, slice-by-4 per lane,
-// then a log-step combine with carry-less multiplications mod the CRC polynomial.
+// The CRC-32 of the output is computed by the same warp while it inflates: a cursor absorbs each
+// 128-byte row of the output as soon as the row is final (CrcCursor below).
 #include "hgpu_internal.h"
 #include <stdlib.h>
 
@@ -81,6 +81,8 @@ struct Prof {
 __device__ uint32_t g_crc_tab[4][256];      // slice-by-4 tables, filled once by crc_init_kernel
 __device__ uint32_t g_xpow_lo[256];         // x^(8 i) mod P            (crc_init2_kernel)
 __device__ uint32_t g_xpow_hi[256];         // x^(8 * 256 i) mod P
+__device__ uint32_t g_crc_tab2[4][256];     // slice-by-4 tables advanced by 124 more zero bytes (x^1024 per word)
+__device__ uint32_t g_xinv_byte[256];       // x^(-8 z) mod P  (x is invertible: P(0) = 1)
 
 __global__ void crc_init_kernel()
 {
@@ -325,6 +327,128 @@ __device__ uint32_t warp_crc32(const uint32_t (*tab)[256], const uint8_t *out, u
     return __shfl_sync(0xffffffffu, crc, 0);
 }
 
+// predicated accesses (straight-line code: `if (c) x = *p` would become a divergent branch).
+// G: global memory (ld/st.global); otherwise generic (the CTA kernel runs the uniform decoder on a
+// shared-memory window).
+template <bool G>
+__device__ __forceinline__ uint32_t ld32_if(const uint8_t *a, bool c)
+{
+    uint32_t v;
+    if (G) asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\tmov.u32 %0, 0;\n\t@q ld.global.u32 %0, [%1];\n\t}" : "=r"(v) : "l"(a), "r"((uint32_t)c) : "memory");
+    else asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\tmov.u32 %0, 0;\n\t@q ld.u32 %0, [%1];\n\t}" : "=r"(v) : "l"(a), "r"((uint32_t)c) : "memory");
+    return v;
+}
+template <bool G>
+__device__ __forceinline__ void st32_if(uint8_t *a, uint32_t v, bool c)
+{
+    if (G) asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.global.u32 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"((uint32_t)c) : "memory");
+    else asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.u32 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"((uint32_t)c) : "memory");
+}
+template <bool G>
+__device__ __forceinline__ void st8_if(uint8_t *a, uint32_t v, bool c)
+{
+    if (G) asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.global.u8 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"((uint32_t)c) : "memory");
+    else asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.u8 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"((uint32_t)c) : "memory");
+}
+// the literal emit of bgzf_huff.cuh
+__device__ __forceinline__ void gst8_if(uint8_t *a, uint32_t v, uint32_t c) { st8_if<false>(a, v, c != 0); }
+
+// ---------------------------------------------------------------------------------------------
+// CRC-32 of a member's output, absorbed while it is being written.
+//
+// The output is read in 128-byte rows aligned to their address (one cache line, one coalesced
+// 32-bit load per lane), each row as soon as every byte in it is final and still hot in L1/L2.
+// Lane-strided Horner form as in cta_crc32: lane l absorbs word l of every row and advances its
+// sum by x^1024 per row (the tables in shared memory are g_crc_tab2).  The message starts at byte
+// m0 of row 0: bytes before it are read as zero (a leading zero does not change a CRC without
+// its initial value), and its first four bytes are complemented, which stands for that initial
+// value.  At the end the last row is zero-padded by z bytes; lane l's sum times x^(-32 l), summed
+// over the lanes, is the register after the padded message, and x^(-8 z) takes the padding out.
+// Words at the member's edges are read bytewise: the bytes around a member belong to other warps
+// and may lie outside the allocation.
+// ---------------------------------------------------------------------------------------------
+struct CrcCursor {
+    const uint32_t *tab;      // g_crc_tab2 in shared memory
+    const uint8_t *row0;      // the member's output rounded down to 128 bytes
+    uint32_t m0;              // member start inside row 0
+    uint32_t next;            // first row not absorbed yet
+    uint32_t acc;             // this lane's Horner sum
+};
+
+__device__ __forceinline__ uint32_t crc_step4(const uint32_t *tab, uint32_t v)
+{
+    return tab[3 * 256 + (v & 0xff)] ^ tab[2 * 256 + ((v >> 8) & 0xff)] ^ tab[256 + ((v >> 16) & 0xff)] ^ tab[v >> 24];
+}
+
+__device__ __forceinline__ uint32_t ldg32(const uint8_t *a) { uint32_t v; asm volatile("ld.global.u32 %0, [%1];" : "=r"(v) : "l"(a) : "memory"); return v; }
+__device__ __forceinline__ uint32_t ldg8(const uint8_t *a) { uint32_t v; asm volatile("ld.global.u8 %0, [%1];" : "=r"(v) : "l"(a) : "memory"); return v; }
+
+__device__ __forceinline__ void crc_begin(CrcCursor &c, const uint32_t *tab, const uint8_t *out)
+{
+    const uintptr_t a = reinterpret_cast<uintptr_t>(out);
+    c.tab = tab;
+    c.row0 = reinterpret_cast<const uint8_t *>(a & ~(uintptr_t)127);
+    c.m0 = (uint32_t)(a & 127);
+    c.next = 0;
+    c.acc = 0;
+}
+
+// word at row offset q: member bytes below lim (row coordinates), zero elsewhere, the first four message bytes complemented
+__device__ __forceinline__ uint32_t crc_edge_word(const CrcCursor &c, uint32_t q, uint32_t lim)
+{
+    uint32_t w = 0;
+    if (q >= c.m0 && q + 4u <= lim) w = ldg32(c.row0 + q);
+    else
+        for (uint32_t i = 0; i < 4; i++)
+            if (q + i >= c.m0 && q + i < lim) w |= ldg8(c.row0 + q + i) << (8 * i);
+    const int32_t rel = (int32_t)c.m0 - (int32_t)q;
+    if (rel > -4 && rel < 4) w ^= rel >= 0 ? 0xffffffffu << (8 * rel) : 0xffffffffu >> (-8 * rel);
+    return w;
+}
+
+// absorb rows [c.next, r_end); lim = end of the member's final bytes in row coordinates
+__device__ __forceinline__ void crc_absorb(CrcCursor &c, uint32_t r_end, uint32_t lim)
+{
+    const uint32_t l4 = 4u * hgpu_lane();
+    const uint32_t *tab = c.tab;
+    uint32_t r = c.next, acc = c.acc;
+    const uint32_t ie = min(r_end, lim >> 7);                  // rows wholly below lim
+    for (; r < r_end && r < 2u; r++) acc = crc_step4(tab, acc ^ crc_edge_word(c, 128u * r + l4, lim));
+    for (uint32_t r8 = r; r8 < ie; r8 += 8) {                  // interior rows: up to eight loads in flight, one round trip
+        const uint8_t *p = c.row0 + 128u * r8 + l4;
+        uint32_t w[8];
+#pragma unroll
+        for (uint32_t k = 0; k < 8; k++) w[k] = ld32_if<true>(p + 128u * k, r8 + k < ie);
+#pragma unroll
+        for (uint32_t k = 0; k < 8; k++)
+            if (r8 + k < ie) acc = crc_step4(tab, acc ^ w[k]);
+    }
+    r = max(r, ie);
+    for (; r < r_end; r++) acc = crc_step4(tab, acc ^ crc_edge_word(c, 128u * r + l4, lim));
+    c.acc = acc;
+    c.next = r;
+}
+
+// the member's bytes [0, f) are final: absorb the whole rows among them.  Warp-uniform; the
+// caller has made the bytes visible to the warp (__syncwarp).
+__device__ __forceinline__ void crc_advance(CrcCursor &c, uint32_t f)
+{
+    const uint32_t lim = c.m0 + f;
+    if ((lim >> 7) > c.next) crc_absorb(c, lim >> 7, lim);
+}
+
+// CRC-32 of the member's n bytes
+__device__ uint32_t crc_finish(CrcCursor &c, uint32_t n)
+{
+    const uint32_t lim = c.m0 + n;
+    const uint32_t rows = (max(lim, c.m0 + 4u) + 127u) >> 7;     // the complemented bytes may reach past the data
+    crc_absorb(c, rows, lim);
+    uint32_t s = multmodp(g_xinv_byte[4u * hgpu_lane()], c.acc);
+#pragma unroll
+    for (int d = 16; d; d >>= 1) s ^= __shfl_xor_sync(0xffffffffu, s, d);
+    return ~multmodp(g_xinv_byte[128u * rows - lim], s);
+}
+
 // ---------------------------------------------------------------------------------------------
 // LZ77 match execution.
 //
@@ -333,74 +457,80 @@ __device__ uint32_t warp_crc32(const uint32_t (*tab)[256], const uint8_t *out, u
 // executed OUT OF ORDER inside the batch.  Destinations inside a batch are ascending and
 // disjoint, so the earlier records a match reads from form one index range, found with two
 // 5-step binary searches over the lanes (shuffles) and kept as a 32-bit dependency mask.  Then,
-// in rounds, every record whose dependencies are done is cut into pieces of <= 32 bytes in a
-// shared-memory piece table and all those pieces are executed together: lane i moves byte i of
-// each piece (coalesced), and all loads of a chunk of GRP pieces are issued before any store.
-// The number of L2 round trips per batch is the depth of its dependency chain (1-4 for sorted
-// BAM), not the number of matches.  Overlapping matches (dist < len, run-length style) are rare
-// and take a separate cooperative path with a per-byte modulo.
+// in rounds, every record whose dependencies are done is executed.  The number of L2 round trips
+// per batch is the depth of its dependency chain (1-4 for sorted BAM), not the number of matches.
 //
-// piece = { dst:16 | plen:6<<16 ,  src }      (offsets into the member's output)
+// A round's ready matches that do not overlap their own source are laid end to end in one space
+// of destination words (4-byte aligned words that hold at least one byte of the match; an
+// exclusive scan of the per-match word counts), and the warp walks that space 32 words at a time:
+// lane j finds its match by a 5-step search over the inclusive scan, funnel-shifts the word from
+// the aligned source words in front of it (the upper one is usually the next lane's lower one)
+// and stores it whole, or bytewise where the word is shared with a literal or another match.
+// Lanes on one match touch the same one or two cache lines.  The loads of the next 32 words are
+// issued before the current ones are first used (load_slot returns with its loads in flight), so a
+// round costs about one L2 round trip however many chunks it has: nothing a round stores is read
+// in that round.
+// Overlapping matches (dist < len, run-length style) are rare and take a separate cooperative
+// path with a per-byte modulo.
 // ---------------------------------------------------------------------------------------------
-#ifndef GRP_N
-#define GRP_N 4
-#endif
-constexpr int GRP = GRP_N;
-
 __device__ __forceinline__ uint32_t low_mask(uint32_t n) { return n >= 32u ? 0xffffffffu : (1u << n) - 1u; }
 
-// predicated global-memory accesses (straight-line code: `if (c) x = *p` would become a divergent branch)
-__device__ __forceinline__ uint32_t gld8_if(const uint8_t *a, uint32_t c)
-{ uint32_t v; asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\tmov.u32 %0, 0;\n\t@q ld.u8 %0, [%1];\n\t}" : "=r"(v) : "l"(a), "r"(c) : "memory"); return v; }
-__device__ __forceinline__ uint32_t gld32_if(const uint8_t *a, uint32_t c)
-{ uint32_t v; asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\tmov.u32 %0, 0;\n\t@q ld.u32 %0, [%1];\n\t}" : "=r"(v) : "l"(a), "r"(c) : "memory"); return v; }
-__device__ __forceinline__ void gst8_if(uint8_t *a, uint32_t v, uint32_t c)
-{ asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.u8 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"(c) : "memory"); }
-__device__ __forceinline__ void gst32_if(uint8_t *a, uint32_t v, uint32_t c)
-{ asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.u32 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"(c) : "memory"); }
+struct WordSlot {
+    uint32_t d;               // destination word, from the aligned base
+    uint32_t lo, hi;          // aligned source words (hi: 0 when the next lane's lo is meant)
+    uint32_t f;               // [3:0] bytes of the word that belong to the match (0xf: all), [8:4] source shift,
+                              // [9] the upper source word is the next lane's lower one
+};
 
-// One match, one lane: d[0..n) = s[0..n), no overlap (dist >= len).  Aligned 32-bit stores with a
-// funnel-shifted source, every load of a chunk (<= 32 bytes) issued before its stores: a chunk costs one
-// round trip to L2, and the lanes of a round pay it together.  act = 0: the lane moves nothing.
-__device__ __forceinline__ void lane_copy(uint8_t *d, const uint8_t *s, uint32_t n, uint32_t act)
+// word `slot` of the round's destination-word space.  inc: inclusive scan of the word counts;
+// wb = (first word of the lane's match) - 4 * (words in front of it); u0 = its destination; ld = len | dist << 16
+template <bool G>
+__device__ __forceinline__ WordSlot load_slot(const uint8_t *ob, uint32_t inc, uint32_t wb, uint32_t u0, uint32_t ld,
+                                              uint32_t slot, uint32_t T)
 {
-    if (!act) n = 0;
-    uint32_t h = (0u - (uint32_t)reinterpret_cast<uintptr_t>(d)) & 3u;
-    if (h > n) h = n;
-    const uint32_t nw = (n - h) >> 2, tl = (n - h) & 3u;
-    const uint8_t *ts = s + h + 4u * nw;
-    uint8_t *td = d + h + 4u * nw;
-    const uint32_t hb0 = gld8_if(s, h > 0), hb1 = gld8_if(s + 1, h > 1), hb2 = gld8_if(s + 2, h > 2);
-    const uint32_t tb0 = gld8_if(ts, tl > 0), tb1 = gld8_if(ts + 1, tl > 1), tb2 = gld8_if(ts + 2, tl > 2);
-    uint8_t *dw = d + h;
-    const uint8_t *sw = s + h;
-    const uint32_t sh = ((uint32_t)reinterpret_cast<uintptr_t>(sw) & 3u) * 8u;
-    const uint8_t *sa = sw - (reinterpret_cast<uintptr_t>(sw) & 3);
-    uint32_t rem = nw;
-    uint32_t W0 = gld32_if(sa, rem > 0);
-    while (rem) {
-        // the word behind the last needed one is read only when the source is misaligned (it then lies inside the match)
-        const uint32_t W1 = gld32_if(sa + 4, rem > 1 || sh), W2 = gld32_if(sa + 8, rem > 2 || (rem > 1 && sh)), W3 = gld32_if(sa + 12, rem > 3 || (rem > 2 && sh)),
-                       W4 = gld32_if(sa + 16, rem > 4 || (rem > 3 && sh)), W5 = gld32_if(sa + 20, rem > 5 || (rem > 4 && sh)), W6 = gld32_if(sa + 24, rem > 6 || (rem > 5 && sh)),
-                       W7 = gld32_if(sa + 28, rem > 7 || (rem > 6 && sh)), W8 = gld32_if(sa + 32, rem > 8 || (rem > 7 && sh));
-        gst32_if(dw, __funnelshift_r(W0, W1, sh), 1);
-        gst32_if(dw + 4, __funnelshift_r(W1, W2, sh), rem > 1);
-        gst32_if(dw + 8, __funnelshift_r(W2, W3, sh), rem > 2);
-        gst32_if(dw + 12, __funnelshift_r(W3, W4, sh), rem > 3);
-        gst32_if(dw + 16, __funnelshift_r(W4, W5, sh), rem > 4);
-        gst32_if(dw + 20, __funnelshift_r(W5, W6, sh), rem > 5);
-        gst32_if(dw + 24, __funnelshift_r(W6, W7, sh), rem > 6);
-        gst32_if(dw + 28, __funnelshift_r(W7, W8, sh), rem > 7);
-        W0 = W8; sa += 32; dw += 32;
-        rem = rem > 8 ? rem - 8 : 0;
-    }
-    gst8_if(d, hb0, h > 0); gst8_if(d + 1, hb1, h > 1); gst8_if(d + 2, hb2, h > 2);
-    gst8_if(td, tb0, tl > 0); gst8_if(td + 1, tb1, tl > 1); gst8_if(td + 2, tb2, tl > 2);
+    const uint32_t lane = hgpu_lane();
+    uint32_t k = 0;                                            // owner: the number of matches ending at or before slot
+#pragma unroll
+    for (int st = 16; st >= 1; st >>= 1)
+        if (__shfl_sync(0xffffffffu, inc, k + st - 1) <= slot) k += st;
+    const uint32_t D = __shfl_sync(0xffffffffu, wb, k) + 4u * slot;
+    const uint32_t a0 = __shfl_sync(0xffffffffu, u0, k), l_d = __shfl_sync(0xffffffffu, ld, k);
+    const uint32_t kn = __shfl_down_sync(0xffffffffu, k, 1);
+    const bool valid = slot < T;
+    const uint32_t dist = l_d >> 16;
+    const uint32_t a = max(D, a0), b = min(D + 4u, a0 + (l_d & 0xffffu));     // the match's bytes in this word
+    const int32_t S = (int32_t)(D - dist), S0 = S & ~3, sh = (S & 3) * 8;      // S >= -3: the source starts at >= 0
+    // only words that hold source bytes [a - dist, b - dist) are touched
+    const bool from_next = lane < 31 && kn == k && slot + 1 < T;               // the next lane's lower word is this one's upper
+    const bool need_lo = valid && S0 + 4 > (int32_t)(a - dist);
+    const bool need_hi = valid && sh != 0 && S0 + 4 < (int32_t)(b - dist) && !from_next;
+    WordSlot w;
+    w.d = D;
+    w.lo = ld32_if<G>(ob + S0, need_lo);
+    w.hi = ld32_if<G>(ob + S0 + 4, need_hi);
+    const uint32_t m = valid ? ((1u << (b - D)) - 1u) & ~((1u << (a - D)) - 1u) : 0u;
+    w.f = m | (uint32_t)sh << 4 | (from_next ? 1u << 9 : 0u);
+    return w;
 }
 
-__device__ __forceinline__ void exec_batch(uint8_t *out, InflateSmem &s, uint2 rec, uint32_t nrec)
+// the first use of the loaded words: load_slot returns with its loads in flight
+template <bool G>
+__device__ __forceinline__ void store_slot(uint8_t *ob, const WordSlot &w)
 {
-    (void)s;
+    const uint32_t lo_next = __shfl_down_sync(0xffffffffu, w.lo, 1);
+    const uint32_t v = __funnelshift_r(w.lo, (w.f >> 9) ? lo_next : w.hi, (w.f >> 4) & 31u);
+    const uint32_t m = w.f & 15u;
+    const bool part = m != 15u;
+    st32_if<G>(ob + w.d, v, !part);
+    st8_if<G>(ob + w.d, v, part && (m & 1u));
+    st8_if<G>(ob + w.d + 1, v >> 8, part && (m & 2u));
+    st8_if<G>(ob + w.d + 2, v >> 16, part && (m & 4u));
+    st8_if<G>(ob + w.d + 3, v >> 24, part && (m & 8u));
+}
+
+template <bool G>
+__device__ __forceinline__ void exec_batch(uint8_t *out, uint2 rec, uint32_t nrec)
+{
     const uint32_t lane = hgpu_lane();
     const bool have = lane < nrec;
     const uint32_t len = have ? (rec.y & 0xffffu) : 0u, dist = rec.y >> 16;
@@ -421,6 +551,11 @@ __device__ __forceinline__ void exec_batch(uint8_t *out, InflateSmem &s, uint2 r
         }
         if (have && j2 > j1) dep = low_mask(j2) & ~low_mask(j1) & hgpu_lanemask_lt();
     }
+    // destination-word space, in coordinates of the 4-byte aligned base ob
+    const uint32_t mis = (uint32_t)reinterpret_cast<uintptr_t>(out) & 3u;
+    uint8_t *ob = out - mis;
+    const uint32_t u0 = dst + mis;
+    const uint32_t nw = have && !ov ? ((u0 + len + 3u) >> 2) - (u0 >> 2) : 0u;
     uint32_t done = low_mask(nrec) ^ 0xffffffffu;
 #ifdef HGPU_PROFILE
     if (lane == 0) atomicAdd(&g_prof[9], 1ull);
@@ -432,8 +567,25 @@ __device__ __forceinline__ void exec_batch(uint8_t *out, InflateSmem &s, uint2 r
 #ifdef HGPU_PROFILE
         if (lane == 0) { atomicAdd(&g_prof[8], 1ull); atomicAdd(&g_prof[11], (unsigned long long)__popc(Rov)); }
 #endif
-        // every ready match that does not overlap its own source: one lane each, word copies
-        lane_copy(out + (have ? dst : 0u), out + (have ? src : 0u), len, ready && !ov);
+        // every ready match that does not overlap its own source: coalesced word copies
+        const uint32_t cnt = ready ? nw : 0u;
+        uint32_t inc = cnt;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t t = __shfl_up_sync(0xffffffffu, inc, d);
+            if (lane >= (uint32_t)d) inc += t;
+        }
+        const uint32_t T = __shfl_sync(0xffffffffu, inc, 31);
+        const uint32_t wb = (u0 & ~3u) - 4u * (inc - cnt);
+        if (T) {
+            WordSlot cur = load_slot<G>(ob, inc, wb, u0, rec.y, lane, T);
+            for (uint32_t base = 0; base < T; base += 32) {
+                WordSlot nxt = {0u, 0u, 0u, 0u};
+                if (base + 32 < T) nxt = load_slot<G>(ob, inc, wb, u0, rec.y, base + 32 + lane, T);
+                store_slot<G>(ob, cur);
+                cur = nxt;
+            }
+        }
         __syncwarp();
         // overlapping matches of this round: the source is the `dist` bytes before the
         // destination, repeated
@@ -460,7 +612,9 @@ __device__ __forceinline__ void exec_batch(uint8_t *out, InflateSmem &s, uint2 r
 // Serial ("uniform") body decoder: all lanes walk the same bit stream.  Used for small deflate
 // blocks and as the fallback when speculation is not worthwhile.
 // ---------------------------------------------------------------------------------------------
-__device__ int decode_body_uniform(InflateSmem &s, Bits &b, uint8_t *out, uint32_t cap, uint32_t &o)
+// G: out is global memory and crc absorbs it as it becomes final; otherwise crc is null.
+template <bool G>
+__device__ int decode_body_uniform(InflateSmem &s, Bits &b, uint8_t *out, uint32_t cap, uint32_t &o, CrcCursor *crc)
 {
     const uint32_t lane = hgpu_lane();
     uint32_t pend = 0;                             // match records parked in s.rbuf
@@ -487,10 +641,15 @@ __device__ int decode_body_uniform(InflateSmem &s, Bits &b, uint8_t *out, uint32
         __syncwarp();
         if (lane == 0) s.rbuf[pend] = make_uint2(o, len | (dist << 16));
         o += len;
-        if (++pend == 32) { __syncwarp(); exec_batch(out, s, s.rbuf[lane], 32); pend = 0; }
+        if (++pend == 32) {
+            __syncwarp();
+            exec_batch<G>(out, s.rbuf[lane], 32);
+            pend = 0;
+            if (G) crc_advance(*crc, o);                   // literals are stored as they are decoded: all of [0, o) is final
+        }
     }
     __syncwarp();
-    if (pend) exec_batch(out, s, s.rbuf[lane], pend);
+    if (pend) exec_batch<G>(out, s.rbuf[lane], pend);
     __syncwarp();
     if (bits_overrun(b)) return HGPU_BGZF_ERR_ZLIB;
     return HGPU_OK;
@@ -607,14 +766,17 @@ __device__ __forceinline__ void lane_decode(const InflateSmem &s, const uint32_t
 
 // Execute mrec[0..total) in order through the window.  Records are fetched 32 at a time
 // (coalesced) and broadcast with shuffles, so every lane sees the same match.
-__device__ void run_matches(InflateSmem &s, uint8_t *out, const uint2 *mrec, uint32_t total)
+// After a batch every byte in front of the next batch's first destination is final (literals were
+// written by the emit pass, earlier matches are done): the CRC cursor takes it.
+__device__ void run_matches(uint8_t *out, const uint2 *mrec, uint32_t total, CrcCursor &crc)
 {
     const uint32_t lane = hgpu_lane();
     uint2 nx = lane < total ? mrec[lane] : make_uint2(0, 0);
     for (uint32_t base = 0; base < total; base += 32) {
         uint2 rec = nx;
         nx = base + 32 + lane < total ? mrec[base + 32 + lane] : make_uint2(0, 0);      // next batch in flight
-        exec_batch(out, s, rec, total - base < 32u ? total - base : 32u);
+        exec_batch<true>(out, rec, total - base < 32u ? total - base : 32u);
+        if (base + 32 < total) crc_advance(crc, __shfl_sync(0xffffffffu, nx.x, 0));
     }
     __syncwarp();
 }
@@ -632,7 +794,7 @@ constexpr uint32_t MREC_CAP = 65536 / 3 + 64;   // a match yields >= 3 bytes of 
 #ifndef HGPU_NEW_WALK
 __device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const uint32_t *wend, uint32_t body,
                                     uint32_t total, uint8_t *out, uint32_t cap, uint32_t &o, uint2 *mrec,
-                                    uint32_t &end_pos, Prof &pf, uint32_t mcap = MREC_CAP)
+                                    uint32_t &end_pos, CrcCursor &crc, Prof &pf, uint32_t mcap = MREC_CAP)
 {
     const uint32_t lane = hgpu_lane();
     const uint32_t S = (total - body + 31) / 32;
@@ -678,7 +840,7 @@ __device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const
     __syncwarp();
     __threadfence_block();
     pf.mark(2);
-    run_matches(s, out, mrec, tot_m);
+    run_matches(out, mrec, tot_m, crc);
     pf.mark(3);
     o += tot_out;
     end_pos = last;
@@ -688,7 +850,7 @@ __device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const
 #else
 __device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const uint32_t *wend, uint32_t body,
                                     uint32_t total, uint8_t *out, uint32_t cap, uint32_t &o, uint2 *mrec,
-                                    uint32_t &end_pos, Prof &pf, uint32_t mcap = MREC_CAP)
+                                    uint32_t &end_pos, CrcCursor &crc, Prof &pf, uint32_t mcap = MREC_CAP)
 {
     const uint32_t lane = hgpu_lane();
     // 32 sub-ranges cut on word boundaries; every lane walks from PREROLL bits in front of its cut (so that
@@ -750,7 +912,7 @@ __device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const
     __syncwarp();
     __threadfence_block();
     pf.mark(2);
-    run_matches(s, out, mrec, tot_m);
+    run_matches(out, mrec, tot_m, crc);
     pf.mark(3);
     o += tot_out;
     end_pos = last;
@@ -763,7 +925,7 @@ __device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const
 // decoders above.
 // ---------------------------------------------------------------------------------------------
 __device__ int inflate_member(InflateSmem &s, const uint8_t *src, uint32_t slen, uint8_t *out, uint32_t cap,
-                              uint32_t &olen, uint2 *mrec, Prof &pf, uint32_t mcap = MREC_CAP)
+                              uint32_t &olen, uint2 *mrec, CrcCursor &crc, Prof &pf, uint32_t mcap = MREC_CAP)
 {
     const uint32_t lane = hgpu_lane();
     Bits b;
@@ -792,6 +954,7 @@ __device__ int inflate_member(InflateSmem &s, const uint8_t *src, uint32_t slen,
             o += len;
             bits_init(b, src, pos + len, slen);
             __syncwarp();
+            crc_advance(crc, o);
         } else if (type == 1 || type == 2) {
             int rc;
             if (type == 1) {
@@ -868,7 +1031,7 @@ __device__ int inflate_member(InflateSmem &s, const uint8_t *src, uint32_t slen,
             pf.mark(0);
             if (total - body >= PAR_MIN_BITS) {
                 uint32_t end_pos = 0;
-                rc = decode_body_parallel(s, wbase, wend, body, total, out, cap, o, mrec, end_pos, pf, mcap);
+                rc = decode_body_parallel(s, wbase, wend, body, total, out, cap, o, mrec, end_pos, crc, pf, mcap);
                 if (rc) return rc;
                 // continue the uniform reader right after the end-of-block code
                 uint32_t byte = (end_pos - mis_bits) >> 3, bit = (end_pos - mis_bits) & 7;
@@ -876,10 +1039,11 @@ __device__ int inflate_member(InflateSmem &s, const uint8_t *src, uint32_t slen,
                 bits_fill(b);
                 bits_drop(b, bit);
             } else {
-                rc = decode_body_uniform(s, b, out, cap, o);
+                rc = decode_body_uniform<true>(s, b, out, cap, o, &crc);
                 if (rc) return rc;
                 pf.mark(5);
             }
+            crc_advance(crc, o);
         } else
             return HGPU_BGZF_ERR_ZLIB;
         if (final) break;
@@ -910,9 +1074,9 @@ bgzf_inflate_kernel(const uint8_t *__restrict__ in, const uint64_t *__restrict__
                     uint32_t *out_len, int32_t *status, uint32_t *counter, uint2 *mrec_all)
 {
     extern __shared__ __align__(16) uint8_t dyn_smem[];
-    uint32_t (*crc_tab)[256] = reinterpret_cast<uint32_t (*)[256]>(dyn_smem);
+    uint32_t *crc_tab = reinterpret_cast<uint32_t *>(dyn_smem);       // g_crc_tab2: the CRC cursor's row step
     InflateSmem *smem_all = reinterpret_cast<InflateSmem *>(dyn_smem + 4096);
-    for (int i = threadIdx.x; i < 1024; i += blockDim.x) (&crc_tab[0][0])[i] = (&g_crc_tab[0][0])[i];
+    for (int i = threadIdx.x; i < 1024; i += blockDim.x) crc_tab[i] = (&g_crc_tab2[0][0])[i];
     __syncthreads();                                   // the only block-wide barrier: warps are independent below
     InflateSmem &s = smem_all[threadIdx.x >> 5];
     uint2 *mrec = mrec_all + ((size_t)blockIdx.x * INFLATE_WARPS + (threadIdx.x >> 5)) * MREC_CAP;
@@ -935,13 +1099,13 @@ bgzf_inflate_kernel(const uint8_t *__restrict__ in, const uint64_t *__restrict__
             // inflate_block hands zlib block_length-18 bytes: deflate data plus the 8-byte footer
             Prof pf;
             pf.start();
-            rc = inflate_member(s, blk + 18, blen - 18, dst, cap, got, mrec, pf);
+            CrcCursor cc;
+            crc_begin(cc, crc_tab, dst);
+            rc = inflate_member(s, blk + 18, blen - 18, dst, cap, got, mrec, cc, pf);
             if (rc == HGPU_OK) {
-                __syncwarp();
-                __threadfence_block();
                 uint32_t want = blk[blen - 8] | blk[blen - 7] << 8 | blk[blen - 6] << 16 | (uint32_t)blk[blen - 5] << 24;
                 pf.mark(6);
-                uint32_t crc = warp_crc32(crc_tab, dst, got);
+                uint32_t crc = crc_finish(cc, got);
                 if (crc != want) rc = HGPU_BGZF_ERR_CRC;
                 pf.mark(4);
             }
@@ -980,9 +1144,9 @@ gzip_inflate_kernel(const uint8_t *__restrict__ in, const uint64_t *__restrict__
                     uint32_t *out_len, int32_t *status, uint32_t *counter, uint2 *mrec_all)
 {
     extern __shared__ __align__(16) uint8_t dyn_smem[];
-    uint32_t (*crc_tab)[256] = reinterpret_cast<uint32_t (*)[256]>(dyn_smem);
+    uint32_t *crc_tab = reinterpret_cast<uint32_t *>(dyn_smem);       // g_crc_tab2: the CRC cursor's row step
     InflateSmem *smem_all = reinterpret_cast<InflateSmem *>(dyn_smem + 4096);
-    for (int i = threadIdx.x; i < 1024; i += blockDim.x) (&crc_tab[0][0])[i] = (&g_crc_tab[0][0])[i];
+    for (int i = threadIdx.x; i < 1024; i += blockDim.x) crc_tab[i] = (&g_crc_tab2[0][0])[i];
     __syncthreads();
     InflateSmem &s = smem_all[threadIdx.x >> 5];
     uint2 *mrec = mrec_all + ((size_t)blockIdx.x * INFLATE_WARPS + (threadIdx.x >> 5)) * GZ_MREC;
@@ -1003,14 +1167,14 @@ gzip_inflate_kernel(const uint8_t *__restrict__ in, const uint64_t *__restrict__
         else {
             Prof pf;
             pf.start();
-            rc = inflate_member(s, blk + hl, blen - (uint32_t)hl, dst, cap, got, mrec, pf, GZ_MREC);
+            CrcCursor cc;
+            crc_begin(cc, crc_tab, dst);
+            rc = inflate_member(s, blk + hl, blen - (uint32_t)hl, dst, cap, got, mrec, cc, pf, GZ_MREC);
             if (rc == HGPU_OK) {
-                __syncwarp();
-                __threadfence_block();
                 const uint8_t *f = blk + blen - 8;
                 const uint32_t want = f[0] | f[1] << 8 | f[2] << 16 | (uint32_t)f[3] << 24;
                 const uint32_t isize = f[4] | f[5] << 8 | f[6] << 16 | (uint32_t)f[7] << 24;
-                const uint32_t crc = warp_crc32(crc_tab, dst, got);
+                const uint32_t crc = crc_finish(cc, got);
                 if (crc != want || isize != got) rc = HGPU_BGZF_ERR_CRC;
             }
         }

@@ -481,7 +481,6 @@ __device__ void lz_resolve_cta(CtaSmem &cs, uint16_t *deps, uint32_t wa, uint32_
 // multiplied by x^(32 (31 - l)), a warp's by x^(8 * bytes behind its region).
 // crc_std(M) = raw(M with its first four bytes complemented) ^ 0xffffffff.
 // ---------------------------------------------------------------------------------------------
-__device__ uint32_t g_crc_tab2[4][256];     // slice-by-4 tables advanced by 124 more zero bytes (x^1024 per word)
 __device__ uint32_t g_xpow_lane[32];        // x^(32 (31 - l))
 
 __global__ void crc_init2_kernel()
@@ -495,11 +494,10 @@ __global__ void crc_init2_kernel()
     g_xpow_lo[i] = xpow_bytes(i);
     g_xpow_hi[i] = xpow_bytes(256u * i);
     if (i < 32) g_xpow_lane[i] = xpow_bytes(4u * (31u - i));
-}
-
-__device__ __forceinline__ uint32_t crc_step4(const uint32_t *tab, uint32_t v)
-{
-    return tab[3 * 256 + (v & 0xff)] ^ tab[2 * 256 + ((v >> 8) & 0xff)] ^ tab[256 + ((v >> 16) & 0xff)] ^ tab[v >> 24];
+    // x^-1 steps: undo one multiplication by x (multmodp's b step), bit 31 = the x^0 coefficient
+    uint32_t v = 1u << 31;
+    for (uint32_t k = 0; k < 8u * i; k++) v = (v & 0x80000000u) ? ((v ^ 0xEDB88320u) << 1) | 1u : v << 1;
+    g_xinv_byte[i] = v;
 }
 
 __device__ uint32_t cta_crc32(CtaSmem &cs, uint32_t *tabs /* [8][256], dead table buffer */, uint32_t a0, uint32_t n)
@@ -684,7 +682,7 @@ bgzf_inflate_cta_kernel(const uint8_t *__restrict__ in, const uint64_t *__restri
                     bits_fill(b);
                     bits_drop(b, bp & 7);
                     uint32_t o = cs.c.o;
-                    int r2 = decode_body_uniform(cs.s[cur], b, win, cap, o);
+                    int r2 = decode_body_uniform<false>(cs.s[cur], b, win, cap, o, nullptr);
                     if (lane == 0) { cs.c.rc = r2; cs.c.o = o; cs.c.end_pos = mis_bits + bits_pos(b); }
                 }
                 __threadfence_block();

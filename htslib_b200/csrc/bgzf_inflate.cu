@@ -6,19 +6,17 @@
 // DEFLATE itself (RFC 1951) and CRC-32 live in zlib/libdeflate for the reference; here they are
 // written from the RFC for the GPU.
 //
-// Kernel structure (v1 — "uniform decode"): all 32 lanes of the warp walk the Huffman stream in
-// lock step (same bit buffer, table lookups broadcast from shared memory), so every lane knows
-// every token without shuffles; literal bytes are stored by lane 0 and LZ77 matches are copied
-// by the whole warp (lane i moves byte i, i+32, ...).  Decode tables are built by the warp in
+// Kernel structure: the warp parses block headers in lock step and builds the decode tables in
 // parallel (canonical code assignment by __match_any_sync ranks) into shared memory:
-//   litlen: 10-bit root + sub-tables, dist: 8-bit root + sub-tables, 32-bit entries
+//   litlen: 9-bit root + sub-tables, dist: 8-bit root + sub-tables, 32-bit entries
 //     [31:16] value (literal / length base / distance base / sub-table offset)
 //     [15:8]  extra-bit count (or sub-table index bits)
 //     [7:4]   kind   [3:0] code bits consumed
-// The CRC-32 of the output is computed by the same warp while it inflates: a cursor absorbs each
-// 128-byte row of the output as soon as the row is final (CrcCursor below).
+// Large deflate block bodies are decoded speculatively, one sub-range per lane; small ones by all
+// lanes in lock step.  LZ77 matches are executed 32 at a time, out of order inside a batch, with
+// warp-coalesced word copies.  The CRC-32 of the output is computed by the same warp while it
+// inflates: a cursor absorbs each 128-byte row of the output as soon as the row is final.
 #include "hgpu_internal.h"
-#include <stdlib.h>
 
 namespace {
 
@@ -33,8 +31,8 @@ enum : uint32_t { K_BAD = 0, K_LIT = 1, K_LEN = 2, K_SUB = 3, K_DIST = 4, K_EOB 
 #define ENTRY(value, xb, kind, nbits) (((uint32_t)(value) << 16) | ((uint32_t)(xb) << 8) | ((uint32_t)(kind) << 4) | (uint32_t)(nbits))
 constexpr uint32_t BAD_ENTRY = ENTRY(0, 0, K_BAD, 0);
 
-// The three areas behind the decode tables are never live at the same time (table building /
-// lane-parallel decode exchange / match execution), so they share storage.
+// The two areas behind the decode tables are never live at the same time (table building /
+// match execution), so they share storage.
 struct InflateSmem {
     uint32_t lit[LIT_TABLE];
     uint32_t dst[DST_TABLE];
@@ -50,12 +48,10 @@ struct InflateSmem {
         struct {                     // match execution
             uint2 rbuf[32];          // match records parked by the serial decoder
         };
-        struct {                     // CTA-per-block decode: what the 256 sub-range decoders exchange
-            uint32_t x_exit[256];
-            uint32_t x_sum[2][8];
-        };
     };
 };
+// the dynamic shared memory per CTA (4 KiB + INFLATE_WARPS x this) sets the occupancy: 3 CTAs of 7 warps per SM
+static_assert(sizeof(InflateSmem) == 10152, "InflateSmem size sets the inflate kernels' occupancy");
 
 __constant__ uint16_t c_len_base[29] = {3,4,5,6,7,8,9,10,11,13,15,17,19,23,27,31,35,43,51,59,67,83,99,115,131,163,195,227,258};
 __constant__ uint8_t  c_len_xtra[29] = {0,0,0,0,0,0,0,0,1,1,1,1,2,2,2,2,3,3,3,3,4,4,4,4,5,5,5,5,0};
@@ -83,21 +79,6 @@ __device__ uint32_t g_xpow_lo[256];         // x^(8 i) mod P            (crc_ini
 __device__ uint32_t g_xpow_hi[256];         // x^(8 * 256 i) mod P
 __device__ uint32_t g_crc_tab2[4][256];     // slice-by-4 tables advanced by 124 more zero bytes (x^1024 per word)
 __device__ uint32_t g_xinv_byte[256];       // x^(-8 z) mod P  (x is invertible: P(0) = 1)
-
-__global__ void crc_init_kernel()
-{
-    uint32_t i = threadIdx.x;
-    uint32_t c = i;
-    for (int k = 0; k < 8; k++) c = (c >> 1) ^ (0xEDB88320u & (0u - (c & 1)));
-    g_crc_tab[0][i] = c;
-    __syncthreads();
-    uint32_t c1 = g_crc_tab[0][c & 0xff] ^ (c >> 8);
-    g_crc_tab[1][i] = c1;
-    uint32_t c2 = g_crc_tab[0][c1 & 0xff] ^ (c1 >> 8);
-    g_crc_tab[2][i] = c2;
-    uint32_t c3 = g_crc_tab[0][c2 & 0xff] ^ (c2 >> 8);
-    g_crc_tab[3][i] = c3;
-}
 
 // ---------------------------------------------------------------------------------------------
 // Bit reader: warp-uniform, 64-bit buffer refilled with aligned 32-bit words.
@@ -287,6 +268,38 @@ __device__ uint32_t xpow_bytes(uint32_t nbytes)
     return p;
 }
 
+__global__ void crc_init_kernel()
+{
+    uint32_t i = threadIdx.x;
+    uint32_t c = i;
+    for (int k = 0; k < 8; k++) c = (c >> 1) ^ (0xEDB88320u & (0u - (c & 1)));
+    g_crc_tab[0][i] = c;
+    __syncthreads();
+    uint32_t c1 = g_crc_tab[0][c & 0xff] ^ (c >> 8);
+    g_crc_tab[1][i] = c1;
+    uint32_t c2 = g_crc_tab[0][c1 & 0xff] ^ (c1 >> 8);
+    g_crc_tab[2][i] = c2;
+    uint32_t c3 = g_crc_tab[0][c2 & 0xff] ^ (c2 >> 8);
+    g_crc_tab[3][i] = c3;
+}
+
+// g_crc_tab2, g_xpow_lo / hi and g_xinv_byte; reads g_crc_tab, so it runs after crc_init_kernel
+__global__ void crc_init2_kernel()
+{
+    const uint32_t i = threadIdx.x;
+    for (int j = 0; j < 4; j++) {
+        uint32_t v = g_crc_tab[j][i];
+        for (int k = 0; k < 124; k++) v = g_crc_tab[0][v & 0xff] ^ (v >> 8);
+        g_crc_tab2[j][i] = v;
+    }
+    g_xpow_lo[i] = xpow_bytes(i);
+    g_xpow_hi[i] = xpow_bytes(256u * i);
+    // x^-1 steps: undo one multiplication by x (multmodp's b step), bit 31 = the x^0 coefficient
+    uint32_t v = 1u << 31;
+    for (uint32_t k = 0; k < 8u * i; k++) v = (v & 0x80000000u) ? ((v ^ 0xEDB88320u) << 1) | 1u : v << 1;
+    g_xinv_byte[i] = v;
+}
+
 // CRC-32 of out[0..n) by the whole warp.  Caller must have made the bytes visible.
 __device__ uint32_t warp_crc32(const uint32_t (*tab)[256], const uint8_t *out, uint32_t n)
 {
@@ -327,38 +340,28 @@ __device__ uint32_t warp_crc32(const uint32_t (*tab)[256], const uint8_t *out, u
     return __shfl_sync(0xffffffffu, crc, 0);
 }
 
-// predicated accesses (straight-line code: `if (c) x = *p` would become a divergent branch).
-// G: global memory (ld/st.global); otherwise generic (the CTA kernel runs the uniform decoder on a
-// shared-memory window).
-template <bool G>
+// predicated global-memory accesses (straight-line code: `if (c) x = *p` would become a divergent branch)
 __device__ __forceinline__ uint32_t ld32_if(const uint8_t *a, bool c)
 {
     uint32_t v;
-    if (G) asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\tmov.u32 %0, 0;\n\t@q ld.global.u32 %0, [%1];\n\t}" : "=r"(v) : "l"(a), "r"((uint32_t)c) : "memory");
-    else asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\tmov.u32 %0, 0;\n\t@q ld.u32 %0, [%1];\n\t}" : "=r"(v) : "l"(a), "r"((uint32_t)c) : "memory");
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\tmov.u32 %0, 0;\n\t@q ld.global.u32 %0, [%1];\n\t}" : "=r"(v) : "l"(a), "r"((uint32_t)c) : "memory");
     return v;
 }
-template <bool G>
 __device__ __forceinline__ void st32_if(uint8_t *a, uint32_t v, bool c)
 {
-    if (G) asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.global.u32 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"((uint32_t)c) : "memory");
-    else asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.u32 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"((uint32_t)c) : "memory");
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.global.u32 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"((uint32_t)c) : "memory");
 }
-template <bool G>
 __device__ __forceinline__ void st8_if(uint8_t *a, uint32_t v, bool c)
 {
-    if (G) asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.global.u8 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"((uint32_t)c) : "memory");
-    else asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.u8 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"((uint32_t)c) : "memory");
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.global.u8 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"((uint32_t)c) : "memory");
 }
-// the literal emit of bgzf_huff.cuh
-__device__ __forceinline__ void gst8_if(uint8_t *a, uint32_t v, uint32_t c) { st8_if<false>(a, v, c != 0); }
 
 // ---------------------------------------------------------------------------------------------
 // CRC-32 of a member's output, absorbed while it is being written.
 //
 // The output is read in 128-byte rows aligned to their address (one cache line, one coalesced
 // 32-bit load per lane), each row as soon as every byte in it is final and still hot in L1/L2.
-// Lane-strided Horner form as in cta_crc32: lane l absorbs word l of every row and advances its
+// Lane-strided Horner form: lane l absorbs word l of every row and advances its
 // sum by x^1024 per row (the tables in shared memory are g_crc_tab2).  The message starts at byte
 // m0 of row 0: bytes before it are read as zero (a leading zero does not change a CRC without
 // its initial value), and its first four bytes are complemented, which stands for that initial
@@ -418,7 +421,7 @@ __device__ __forceinline__ void crc_absorb(CrcCursor &c, uint32_t r_end, uint32_
         const uint8_t *p = c.row0 + 128u * r8 + l4;
         uint32_t w[8];
 #pragma unroll
-        for (uint32_t k = 0; k < 8; k++) w[k] = ld32_if<true>(p + 128u * k, r8 + k < ie);
+        for (uint32_t k = 0; k < 8; k++) w[k] = ld32_if(p + 128u * k, r8 + k < ie);
 #pragma unroll
         for (uint32_t k = 0; k < 8; k++)
             if (r8 + k < ie) acc = crc_step4(tab, acc ^ w[k]);
@@ -484,7 +487,6 @@ struct WordSlot {
 
 // word `slot` of the round's destination-word space.  inc: inclusive scan of the word counts;
 // wb = (first word of the lane's match) - 4 * (words in front of it); u0 = its destination; ld = len | dist << 16
-template <bool G>
 __device__ __forceinline__ WordSlot load_slot(const uint8_t *ob, uint32_t inc, uint32_t wb, uint32_t u0, uint32_t ld,
                                               uint32_t slot, uint32_t T)
 {
@@ -506,29 +508,27 @@ __device__ __forceinline__ WordSlot load_slot(const uint8_t *ob, uint32_t inc, u
     const bool need_hi = valid && sh != 0 && S0 + 4 < (int32_t)(b - dist) && !from_next;
     WordSlot w;
     w.d = D;
-    w.lo = ld32_if<G>(ob + S0, need_lo);
-    w.hi = ld32_if<G>(ob + S0 + 4, need_hi);
+    w.lo = ld32_if(ob + S0, need_lo);
+    w.hi = ld32_if(ob + S0 + 4, need_hi);
     const uint32_t m = valid ? ((1u << (b - D)) - 1u) & ~((1u << (a - D)) - 1u) : 0u;
     w.f = m | (uint32_t)sh << 4 | (from_next ? 1u << 9 : 0u);
     return w;
 }
 
 // the first use of the loaded words: load_slot returns with its loads in flight
-template <bool G>
 __device__ __forceinline__ void store_slot(uint8_t *ob, const WordSlot &w)
 {
     const uint32_t lo_next = __shfl_down_sync(0xffffffffu, w.lo, 1);
     const uint32_t v = __funnelshift_r(w.lo, (w.f >> 9) ? lo_next : w.hi, (w.f >> 4) & 31u);
     const uint32_t m = w.f & 15u;
     const bool part = m != 15u;
-    st32_if<G>(ob + w.d, v, !part);
-    st8_if<G>(ob + w.d, v, part && (m & 1u));
-    st8_if<G>(ob + w.d + 1, v >> 8, part && (m & 2u));
-    st8_if<G>(ob + w.d + 2, v >> 16, part && (m & 4u));
-    st8_if<G>(ob + w.d + 3, v >> 24, part && (m & 8u));
+    st32_if(ob + w.d, v, !part);
+    st8_if(ob + w.d, v, part && (m & 1u));
+    st8_if(ob + w.d + 1, v >> 8, part && (m & 2u));
+    st8_if(ob + w.d + 2, v >> 16, part && (m & 4u));
+    st8_if(ob + w.d + 3, v >> 24, part && (m & 8u));
 }
 
-template <bool G>
 __device__ __forceinline__ void exec_batch(uint8_t *out, uint2 rec, uint32_t nrec)
 {
     const uint32_t lane = hgpu_lane();
@@ -578,11 +578,11 @@ __device__ __forceinline__ void exec_batch(uint8_t *out, uint2 rec, uint32_t nre
         const uint32_t T = __shfl_sync(0xffffffffu, inc, 31);
         const uint32_t wb = (u0 & ~3u) - 4u * (inc - cnt);
         if (T) {
-            WordSlot cur = load_slot<G>(ob, inc, wb, u0, rec.y, lane, T);
+            WordSlot cur = load_slot(ob, inc, wb, u0, rec.y, lane, T);
             for (uint32_t base = 0; base < T; base += 32) {
                 WordSlot nxt = {0u, 0u, 0u, 0u};
-                if (base + 32 < T) nxt = load_slot<G>(ob, inc, wb, u0, rec.y, base + 32 + lane, T);
-                store_slot<G>(ob, cur);
+                if (base + 32 < T) nxt = load_slot(ob, inc, wb, u0, rec.y, base + 32 + lane, T);
+                store_slot(ob, cur);
                 cur = nxt;
             }
         }
@@ -612,9 +612,7 @@ __device__ __forceinline__ void exec_batch(uint8_t *out, uint2 rec, uint32_t nre
 // Serial ("uniform") body decoder: all lanes walk the same bit stream.  Used for small deflate
 // blocks and as the fallback when speculation is not worthwhile.
 // ---------------------------------------------------------------------------------------------
-// G: out is global memory and crc absorbs it as it becomes final; otherwise crc is null.
-template <bool G>
-__device__ int decode_body_uniform(InflateSmem &s, Bits &b, uint8_t *out, uint32_t cap, uint32_t &o, CrcCursor *crc)
+__device__ int decode_body_uniform(InflateSmem &s, Bits &b, uint8_t *out, uint32_t cap, uint32_t &o, CrcCursor &crc)
 {
     const uint32_t lane = hgpu_lane();
     uint32_t pend = 0;                             // match records parked in s.rbuf
@@ -643,13 +641,13 @@ __device__ int decode_body_uniform(InflateSmem &s, Bits &b, uint8_t *out, uint32
         o += len;
         if (++pend == 32) {
             __syncwarp();
-            exec_batch<G>(out, s.rbuf[lane], 32);
+            exec_batch(out, s.rbuf[lane], 32);
             pend = 0;
-            if (G) crc_advance(*crc, o);                   // literals are stored as they are decoded: all of [0, o) is final
+            crc_advance(crc, o);                           // literals are stored as they are decoded: all of [0, o) is final
         }
     }
     __syncwarp();
-    if (pend) exec_batch<G>(out, s.rbuf[lane], pend);
+    if (pend) exec_batch(out, s.rbuf[lane], pend);
     __syncwarp();
     if (bits_overrun(b)) return HGPU_BGZF_ERR_ZLIB;
     return HGPU_OK;
@@ -711,17 +709,14 @@ __device__ __forceinline__ uint32_t lb_lookup(const uint32_t *table, LaneBits &b
 
 enum : uint32_t { ST_RUN = 0, ST_EOB = 1, ST_BAD = 2 };
 
-// Decode tokens in [start, end).  EMIT=false: count output bytes / matches.  EMIT=true: write
-// literals at out[obase..] and match records at mrec[mbase..]; sets bad_dist on a distance that
-// reaches before the start of the output.
-// EMIT: 0 count only; 1 literals to out[] + {dst, len | dist<<16} records to mrec[]; 2 literals to
-// out[] + a 3-byte record {len-3, dist-1 (15 bits)} parked IN the output at the match's own
-// destination (a match owns >= 3 bytes there) + its destination in the 16-bit list dlist[].
+// Decode tokens in [start, end).  EMIT=0: count output bytes / matches.  EMIT=1: write literals at
+// out[obase..] and {dst, len | dist<<16} match records at mrec[mbase..]; sets bad_dist on a
+// distance that reaches before the start of the output.
 template <int EMIT>
 __device__ __forceinline__ void lane_decode(const InflateSmem &s, const uint32_t *wbase, const uint32_t *wend,
                                             uint32_t start, uint32_t end, uint32_t &exitp, uint32_t &nout,
                                             uint32_t &nmatch, uint32_t &st, uint8_t *out, uint32_t obase,
-                                            uint2 *mrec, uint32_t mbase, bool &bad_dist, uint16_t *dlist = nullptr)
+                                            uint2 *mrec, uint32_t mbase, bool &bad_dist)
 {
     LaneBits b;
     uint32_t n = 0, m = 0, status = ST_RUN;
@@ -744,17 +739,10 @@ __device__ __forceinline__ void lane_decode(const InflateSmem &s, const uint32_t
             uint32_t xd = (d >> 8) & 0xff;
             uint32_t dist = (d >> 16) + ((uint32_t)b.buf & ((1u << xd) - 1));
             b.buf >>= xd; b.cnt -= (int)xd;
-            if (EMIT == 1) {
+            if (EMIT) {
                 uint32_t dstpos = obase + n;
                 if (dist > dstpos) bad_dist = true;
                 mrec[mbase + m] = make_uint2(dstpos, len | (dist << 16));
-            } else if (EMIT == 2) {
-                uint32_t dstpos = obase + n;
-                if (dist > dstpos) bad_dist = true;
-                out[dstpos] = (uint8_t)(len - 3);
-                out[dstpos + 1] = (uint8_t)(dist - 1);
-                out[dstpos + 2] = (uint8_t)((dist - 1) >> 8);
-                dlist[mbase + m] = (uint16_t)dstpos;
             }
             n += len; m++;
         } else if (kind == K_EOB) { status = ST_EOB; break; }
@@ -775,23 +763,17 @@ __device__ void run_matches(uint8_t *out, const uint2 *mrec, uint32_t total, Crc
     for (uint32_t base = 0; base < total; base += 32) {
         uint2 rec = nx;
         nx = base + 32 + lane < total ? mrec[base + 32 + lane] : make_uint2(0, 0);      // next batch in flight
-        exec_batch<true>(out, rec, total - base < 32u ? total - base : 32u);
+        exec_batch(out, rec, total - base < 32u ? total - base : 32u);
         if (base + 32 < total) crc_advance(crc, __shfl_sync(0xffffffffu, nx.x, 0));
     }
     __syncwarp();
 }
-
-#include "bgzf_huff.cuh"
 
 constexpr uint32_t PAR_MIN_BITS = 32 * 96;      // below this a deflate block is decoded serially
 constexpr uint32_t MREC_CAP = 65536 / 3 + 64;   // a match yields >= 3 bytes of a <= 64 KiB member
 
 // Parallel decode of one Huffman block body starting at bit `body` of the member (bit 0 = first
 // bit of word wbase[0], i.e. positions include the alignment offset).  total = end of input.
-// The warp kernel uses the register-buffered bit reader below rather than the position-based branch-free walk of
-// bgzf_huff.cuh, whose two stream loads per symbol come from global memory here, not from a staged copy.
-// -DHGPU_NEW_WALK selects the other (A/B with tools/prof_inflate.py).
-#ifndef HGPU_NEW_WALK
 __device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const uint32_t *wend, uint32_t body,
                                     uint32_t total, uint8_t *out, uint32_t cap, uint32_t &o, uint2 *mrec,
                                     uint32_t &end_pos, CrcCursor &crc, Prof &pf, uint32_t mcap = MREC_CAP)
@@ -847,82 +829,9 @@ __device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const
     return HGPU_OK;
 }
 
-#else
-__device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const uint32_t *wend, uint32_t body,
-                                    uint32_t total, uint8_t *out, uint32_t cap, uint32_t &o, uint2 *mrec,
-                                    uint32_t &end_pos, CrcCursor &crc, Prof &pf, uint32_t mcap = MREC_CAP)
-{
-    const uint32_t lane = hgpu_lane();
-    // 32 sub-ranges cut on word boundaries; every lane walks from PREROLL bits in front of its cut (so that
-    // it has usually found the true token grid by the time it reaches its own range) and counts from the cut
-    const uint32_t w0 = body >> 5, nwords = ((total + 31u) >> 5) - w0, Sw = (nwords + 31u) / 32u;
-    const uint32_t cut = lane == 0 ? body : min(total, (w0 + lane * Sw) << 5);
-    const uint32_t end = lane == 31 ? total : min(total, (w0 + (lane + 1) * Sw) << 5);
-    uint32_t start = cut, exitp = 0, n = 0, m = 0, st = ST_RUN, rc_ = 0;
-    bool dummy = false;
-    {
-        const uint32_t pre = lane == 0 ? body : max(body, cut - min(cut, PREROLL));
-        uint32_t p0 = cut;
-        huff_walk<0, false, false>(s, 0, wbase, wend, cut, pre, end, cut < end, 0, exitp, n, m, st, rc_, 0, 0, 0, nullptr, dummy, cut, &p0);
-        if (cut < end) start = p0; else exitp = start;
-    }
-    // a lane whose predecessor's exit is not its start walks again from there.  Only lanes up to the first
-    // one that currently ends in an end-of-block code matter.
-    for (int round = 0; round < 34; round++) {
-        const uint32_t prev = __shfl_up_sync(0xffffffffu, exitp, 1);
-        const uint32_t eobs = __ballot_sync(0xffffffffu, st == ST_EOB);
-        const uint32_t Em = eobs ? (uint32_t)__ffs(eobs) - 1u : 32u;
-        const uint32_t ns = lane == 0 ? start : prev;
-        const bool need = ns != start && lane <= Em;
-        if (!__any_sync(0xffffffffu, need)) break;
-        if (need) start = ns;
-        const bool thru = need && start >= end;                  // the predecessor ran through this whole range
-        if (thru) { exitp = start; n = 0; m = 0; st = ST_RUN; }
-        uint32_t e2, n2, m2, s2;
-        huff_walk<0, false, false>(s, 0, wbase, wend, cut, start, end, need && !thru, 0, e2, n2, m2, s2, rc_, 0, 0, 0, nullptr, dummy, start);
-        if (need && !thru) { exitp = e2; n = n2; m = m2; st = s2; }
-    }
-    pf.mark(1);
-    // the chain is now consistent: lane i starts where lane i-1 stopped
-    uint32_t eob = __ballot_sync(0xffffffffu, st == ST_EOB);
-    uint32_t bad = __ballot_sync(0xffffffffu, st == ST_BAD);
-    if (!eob) return HGPU_BGZF_ERR_ZLIB;                       // input ends without an end-of-block code
-    uint32_t E = __ffs(eob) - 1;
-    if (bad & ((2u << E) - 1u)) return HGPU_BGZF_ERR_ZLIB;     // invalid code at or before the end of block
-    uint32_t last = __shfl_sync(0xffffffffu, exitp, E);
-    if (last > total) return HGPU_BGZF_ERR_ZLIB;               // the block ran past the input
-    if (lane > E) { n = 0; m = 0; }
-    // exclusive prefix sums of bytes and matches
-    uint32_t on = n, mn = m;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        uint32_t a = __shfl_up_sync(0xffffffffu, on, d), c = __shfl_up_sync(0xffffffffu, mn, d);
-        if (lane >= (uint32_t)d) { on += a; mn += c; }
-    }
-    uint32_t tot_out = __shfl_sync(0xffffffffu, on, 31), tot_m = __shfl_sync(0xffffffffu, mn, 31);
-    if ((uint64_t)o + tot_out > cap) return HGPU_BGZF_ERR_SPACE;
-    if (tot_m > mcap) return HGPU_BGZF_ERR_ZLIB;           // impossible within 64 KiB of output
-    bool bad_dist = false;
-    {
-        uint32_t e2, n2, m2, st2;
-        huff_walk<3, false, false>(s, 0, wbase, wend, cut, start, end, lane <= E, 0, e2, n2, m2, st2, rc_, 0, o + on - n, mn - m, nullptr, bad_dist,
-                                   0, nullptr, out, mrec);
-    }
-    if (__any_sync(0xffffffffu, bad_dist)) return HGPU_BGZF_ERR_ZLIB;   // distance too far back
-    __syncwarp();
-    __threadfence_block();
-    pf.mark(2);
-    run_matches(out, mrec, tot_m, crc);
-    pf.mark(3);
-    o += tot_out;
-    end_pos = last;
-    return HGPU_OK;
-}
-
-#endif
 // ---------------------------------------------------------------------------------------------
-// One BGZF member: headers + table construction are warp-uniform, bodies go to one of the two
-// decoders above.
+// One BGZF member: headers + table construction are warp-uniform, bodies go to the lane-parallel
+// decoder or, below PAR_MIN_BITS, to the uniform one.
 // ---------------------------------------------------------------------------------------------
 __device__ int inflate_member(InflateSmem &s, const uint8_t *src, uint32_t slen, uint8_t *out, uint32_t cap,
                               uint32_t &olen, uint2 *mrec, CrcCursor &crc, Prof &pf, uint32_t mcap = MREC_CAP)
@@ -1039,7 +948,7 @@ __device__ int inflate_member(InflateSmem &s, const uint8_t *src, uint32_t slen,
                 bits_fill(b);
                 bits_drop(b, bit);
             } else {
-                rc = decode_body_uniform<true>(s, b, out, cap, o, &crc);
+                rc = decode_body_uniform(s, b, out, cap, o, crc);
                 if (rc) return rc;
                 pf.mark(5);
             }
@@ -1182,8 +1091,6 @@ gzip_inflate_kernel(const uint8_t *__restrict__ in, const uint64_t *__restrict__
         if (lane == 0) { status[job] = rc; out_len[job] = rc == HGPU_OK ? got : 0; }
     }
 }
-
-#include "bgzf_inflate_cta.cuh"
 
 __global__ void crc32_chunks_kernel(const uint8_t *buf, size_t len, size_t chunk, uint32_t *partial)
 {
@@ -1650,43 +1557,32 @@ int hgpu_launch_bgzf_inflate(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t 
     if (hgpu_check(cudaSetDevice(ctx->device), "cudaSetDevice")) return HGPU_ERR_CUDA;
     int rc = ensure_crc_tables(ctx, st);
     if (rc) return rc;
-    // The product path is the warp-per-block kernel (as many blocks in flight per SM as occupancy allows,
-    // LZ77 through L2 with per-lane word copies).  HGPU_INFLATE_CTA=1 selects the CTA-per-block kernel
-    // (window in shared memory, 2 blocks per SM) for A/B measurements.
-    static const bool use_warp = !(getenv("HGPU_INFLATE_CTA") && getenv("HGPU_INFLATE_CTA")[0] == '1');
+    // one warp per block, as many blocks in flight per SM as occupancy allows
     static bool attr_set[64];                          // function attributes are per device
     const int dv = ctx->device & 63;
-    const size_t dyn_w = 4096 + INFLATE_WARPS * sizeof(InflateSmem), dyn_c = sizeof(CtaSmem);
+    const size_t dyn_w = 4096 + INFLATE_WARPS * sizeof(InflateSmem);
     if (!attr_set[dv]) {
-        if (hgpu_check(cudaFuncSetAttribute(bgzf_inflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_w), "inflate smem attr") ||
-            hgpu_check(cudaFuncSetAttribute(bgzf_inflate_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_c), "inflate smem attr"))
+        if (hgpu_check(cudaFuncSetAttribute(bgzf_inflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_w), "inflate smem attr"))
             return HGPU_ERR_CUDA;
         attr_set[dv] = true;
     }
     int per_sm = 0;
-    if (use_warp) {
-        if (hgpu_check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bgzf_inflate_kernel, 32 * INFLATE_WARPS, dyn_w), "inflate occupancy"))
-            return HGPU_ERR_CUDA;
-    } else if (hgpu_check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bgzf_inflate_cta_kernel, CTA_T, dyn_c), "inflate occupancy"))
+    if (hgpu_check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bgzf_inflate_kernel, 32 * INFLATE_WARPS, dyn_w), "inflate occupancy"))
         return HGPU_ERR_CUDA;
     if (per_sm < 1) per_sm = 1;
-    const uint32_t units = use_warp ? (n + INFLATE_WARPS - 1) / INFLATE_WARPS : n;
+    const uint32_t units = (n + INFLATE_WARPS - 1) / INFLATE_WARPS;
     uint32_t full_grid = (uint32_t)ctx->sm_count * (uint32_t)per_sm, grid = full_grid;
     if (grid > units) grid = units;
     uint32_t *counter = hgpu_take_counter(ctx, st);
     if (!counter) return HGPU_ERR_CUDA;
-    // match-record scratch, one slot per resident warp (CTA), sized for the full grid so concurrent
+    // match-record scratch, one slot per resident warp, sized for the full grid so concurrent
     // launches on other streams (the pipelined host path) can share the same layout
-    const uint32_t slots = use_warp ? full_grid * INFLATE_WARPS : full_grid;
+    const uint32_t slots = full_grid * INFLATE_WARPS;
     rc = hgpu_ensure_mrec(ctx, (size_t)slots * MREC_CAP * sizeof(uint2) * 3);
     if (rc) return rc;
     uint2 *mrec = reinterpret_cast<uint2 *>(ctx->d_mrec) + (size_t)(ctx->next_counter % 3) * slots * MREC_CAP;
-    if (use_warp)
-        bgzf_inflate_kernel<<<grid, 32 * INFLATE_WARPS, dyn_w, st>>>(d_in, d_in_off, d_in_len, n, d_out, d_out_off, d_out_cap,
-                                                                     d_out_len, d_status, counter, mrec);
-    else
-        bgzf_inflate_cta_kernel<<<grid, CTA_T, dyn_c, st>>>(d_in, d_in_off, d_in_len, n, d_out, d_out_off, d_out_cap,
-                                                            d_out_len, d_status, counter, mrec);
+    bgzf_inflate_kernel<<<grid, 32 * INFLATE_WARPS, dyn_w, st>>>(d_in, d_in_off, d_in_len, n, d_out, d_out_off, d_out_cap,
+                                                                 d_out_len, d_status, counter, mrec);
     hgpu_count_launch();
     return hgpu_check(cudaGetLastError(), "inflate launch");
 }
@@ -1720,17 +1616,6 @@ int hgpu_launch_gzip_inflate(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t 
     gzip_inflate_kernel<<<grid, 32 * INFLATE_WARPS, dyn_w, st>>>(d_in, d_in_off, d_in_len, n, d_out, d_out_off, d_out_cap, d_out_len, d_status, counter, mrec);
     hgpu_count_launch();
     return hgpu_check(cudaGetLastError(), "gzip inflate launch");
-}
-
-extern "C" int hgpu_debug_p2(int job, unsigned int *out)
-{
-#ifdef HGPU_PROFILE
-    if (out) return cudaMemcpyFromSymbol(out, g_dbg, sizeof(uint32_t) * 6 * 256) == cudaSuccess ? 0 : -1;
-    return cudaMemcpyToSymbol(g_dbg_job, &job, sizeof(int)) == cudaSuccess ? 0 : -1;
-#else
-    (void)job; (void)out;
-    return -1;
-#endif
 }
 
 extern "C" int hgpu_debug_profile(unsigned long long *out8)

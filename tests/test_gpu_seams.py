@@ -1,12 +1,10 @@
 """GPU parity of the batching seams a patched htslib calls (INTEGRATION.md B3): hgpu_bgzf_inflate_blocks_host and
-hgpu_bgzf_inflate_jobs_host with ragged slots, zero-length blocks in mid-batch and errors in order; the two inflate
-kernels against each other; untrusted CRAM size fields; two contexts in one process (per-device function
-attributes).  bgzf.c:1010-1093, :1373-1384, :1598-1738; cram/cram_io.c:1576-1754."""
+hgpu_bgzf_inflate_jobs_host with ragged slots, zero-length blocks in mid-batch and errors in order; untrusted CRAM
+size fields; two contexts in one process (per-device function attributes).  bgzf.c:1010-1093, :1373-1384,
+:1598-1738; cram/cram_io.c:1576-1754."""
 import ctypes as C
 import os
 import random
-import subprocess
-import sys
 import zlib
 import numpy as np
 import pytest
@@ -14,7 +12,6 @@ import htslib_b200 as H
 from _libs import GOLD, BGZF_EOF, bgzf_block, orc_bgzf_inflate_block
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -102,14 +99,6 @@ def test_jobs_host_like_bgzf_mt_reader(ctx):
             assert int(st[i]) == wst, i
             if wst == 0:
                 assert int(ulen[i]) == len(wdata) and unc[i][:len(wdata)].tobytes() == wdata, i
-
-
-def test_both_inflate_kernels_pass_the_bgzf_suite():
-    """the product path is the warp-per-block kernel; the CTA-per-block kernel (HGPU_INFLATE_CTA=1) must give the same results"""
-    env = dict(os.environ, HGPU_INFLATE_CTA="1")
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", "test_gpu_bgzf.py"), "-x", "-q", "-m", "gpu"],
-                       env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=900, cwd=ROOT)
-    assert r.returncode == 0, r.stdout.decode()[-3000:]
 
 
 def test_cram_blocks_with_absurd_size_fields(ctx):

@@ -26,7 +26,7 @@ def raw(rep):
     return rows[0], rows[1], rows[2:]
 
 
-for name in ("inflate", "rans", "bam", "tok3", "fast32", "tile4", "inflate_cta", "cram_records"):
+for name in ("inflate", "rans", "bam", "tok3", "fast32", "tile4", "cram_records"):
     rep = os.path.join(G, "%s_%s.ncu-rep" % (tag, name))
     if not os.path.exists(rep):
         continue

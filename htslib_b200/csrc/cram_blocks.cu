@@ -9,15 +9,7 @@
 // gzip_inflate_kernel; BZIP2 / LZMA blocks are reported HGPU_CRAM_UNSUPPORTED and stay with the host library.
 #include "hgpu_internal.h"
 #include <vector>
-#include <new>
 #include <string.h>
-
-extern "C" int hgpu_rans4x8_decode_batch_dev(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off,
-        const uint32_t *d_in_len, uint32_t n, uint8_t *d_out, const uint64_t *d_out_off, const uint32_t *d_out_len,
-        uint32_t *d_got_len, int32_t *d_status, void *stream);
-extern "C" int hgpu_arith_decode_batch_dev(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off,
-        const uint32_t *d_in_len, uint32_t n, uint8_t *d_out, const uint64_t *d_out_off, const uint32_t *d_out_len,
-        uint32_t *d_got_len, int32_t *d_status, uint32_t max_out_len, void *stream);
 
 // Size fields of a CRAM block are untrusted.  A block that claims more than this is refused on its own
 // (HGPU_CRAM_ERR_DECODE, what the reference's cram_uncompress_block returns when its malloc fails); blocks above
@@ -122,67 +114,56 @@ static int cram_uncompress_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t fil
         else { n6++; if (b.uncomp_size > max6 && b.uncomp_size <= BIG_BLOCK) max6 = b.uncomp_size; }
     }
     for (uint32_t i = 0; i < n; i++) { coff[i] = blocks[i].data_off - blocks[i].hdr_len; clen[i] = blocks[i].hdr_len + blocks[i].comp_size; }
-    auto up = [](uint64_t x) { return (x + 255) & ~(uint64_t)255; };
-    const uint64_t o_file = 0, o_out = o_file + up(file_len + 8), o_jio = o_out + up(out_span + 8), o_joo = o_jio + up((uint64_t)nj * 8),
-                   o_jil = o_joo + up((uint64_t)nj * 8), o_jol = o_jil + up((uint64_t)nj * 4), o_got = o_jol + up((uint64_t)nj * 4),
-                   o_st = o_got + up((uint64_t)nj * 4), o_coff = o_st + up((uint64_t)nj * 4), o_clen = o_coff + up((uint64_t)n * 8),
-                   o_crc = o_clen + up((uint64_t)n * 4), total = o_crc + up((uint64_t)n * 4);
-    int rc = hgpu_ensure_stage(ctx, total + 256);
+    StageLayout L;
+    const auto s_file = L.seg(file_len + 8), s_out = L.seg(out_span + 8), s_jio = L.seg((size_t)nj * 8), s_joo = L.seg((size_t)nj * 8),
+               s_jil = L.seg((size_t)nj * 4), s_jol = L.seg((size_t)nj * 4), s_got = L.seg((size_t)nj * 4), s_st = L.seg((size_t)nj * 4),
+               s_coff = L.seg((size_t)n * 8), s_clen = L.seg((size_t)n * 4), s_crc = L.seg((size_t)n * 4);
+    int rc = hgpu_stage_ensure(ctx, L);
     if (rc) return rc;
-    uint8_t *base = ctx->d_stage;
     cudaStream_t s = ctx->stream;
-    if (hgpu_check(cudaMemcpyAsync(base + o_file, file, file_len, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(base + o_coff, coff.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(base + o_clen, clen.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-    if (nj) {
-        if (hgpu_check(cudaMemcpyAsync(base + o_jio, jio.data(), (size_t)nj * 8, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(base + o_joo, joo.data(), (size_t)nj * 8, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(base + o_jil, jil.data(), (size_t)nj * 4, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(base + o_jol, jol.data(), (size_t)nj * 4, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-    }
-    rc = hgpu_launch_crc32_batch(ctx, base + o_file, (const uint64_t *)(base + o_coff), (const uint32_t *)(base + o_clen), n,
-                                 (uint32_t *)(base + o_crc), s);
+    if (hgpu_h2d(L.at(s_file), file, file_len, s) || hgpu_h2d(L.at(s_coff), coff.data(), (size_t)n * 8, s) ||
+        hgpu_h2d(L.at(s_clen), clen.data(), (size_t)n * 4, s) || hgpu_h2d(L.at(s_jio), jio.data(), (size_t)nj * 8, s) ||
+        hgpu_h2d(L.at(s_joo), joo.data(), (size_t)nj * 8, s) || hgpu_h2d(L.at(s_jil), jil.data(), (size_t)nj * 4, s) ||
+        hgpu_h2d(L.at(s_jol), jol.data(), (size_t)nj * 4, s)) return HGPU_ERR_CUDA;
+    uint8_t *d_file = L.at(s_file), *d_out = L.at(s_out);
+    rc = hgpu_launch_crc32_batch(ctx, d_file, L.at<uint64_t>(s_coff), L.at<uint32_t>(s_clen), n, L.at<uint32_t>(s_crc), s);
     if (rc) return rc;
-    const uint64_t *d_jio = (const uint64_t *)(base + o_jio), *d_joo = (const uint64_t *)(base + o_joo);
-    const uint32_t *d_jil = (const uint32_t *)(base + o_jil), *d_jol = (const uint32_t *)(base + o_jol);
-    uint32_t *d_got = (uint32_t *)(base + o_got);
-    int32_t *d_st = (int32_t *)(base + o_st);
+    const uint64_t *d_jio = L.at<uint64_t>(s_jio), *d_joo = L.at<uint64_t>(s_joo);
+    const uint32_t *d_jil = L.at<uint32_t>(s_jil), *d_jol = L.at<uint32_t>(s_jol);
+    uint32_t *d_got = L.at<uint32_t>(s_got);
+    int32_t *d_st = L.at<int32_t>(s_st);
     if (n4) {
-        rc = hgpu_rans4x8_decode_batch_dev(ctx, base + o_file, d_jio, d_jil, n4, base + o_out, d_joo, d_jol, d_got, d_st, s);
+        rc = hgpu_rans4x8_decode_batch_dev(ctx, d_file, d_jio, d_jil, n4, d_out, d_joo, d_jol, d_got, d_st, s);
         if (rc) return rc;
     }
     std::vector<uint32_t> nomem;                                              // big blocks whose own scratch could not be had
     if (n5 - big5) {
-        rc = hgpu_launch_rans_nx16(ctx, base + o_file, d_jio + n4, d_jil + n4, n5 - big5, base + o_out, d_joo + n4, d_jol + n4,
+        rc = hgpu_launch_rans_nx16(ctx, d_file, d_jio + n4, d_jil + n4, n5 - big5, d_out, d_joo + n4, d_jol + n4,
                                    d_got + n4, d_st + n4, max5, s);
         if (rc) return rc;
     }
     for (uint32_t k = n4 + n5 - big5; k < n4 + n5; k++) {
-        rc = hgpu_launch_rans_nx16(ctx, base + o_file, d_jio + k, d_jil + k, 1, base + o_out, d_joo + k, d_jol + k, d_got + k, d_st + k, jol[k], s);
+        rc = hgpu_launch_rans_nx16(ctx, d_file, d_jio + k, d_jil + k, 1, d_out, d_joo + k, d_jol + k, d_got + k, d_st + k, jol[k], s);
         if (rc == HGPU_ERR_NOMEM) nomem.push_back(k); else if (rc) return rc;
     }
     if (n6 - big6) {
-        rc = hgpu_arith_decode_batch_dev(ctx, base + o_file, d_jio + n4 + n5, d_jil + n4 + n5, n6 - big6, base + o_out, d_joo + n4 + n5,
+        rc = hgpu_arith_decode_batch_dev(ctx, d_file, d_jio + n4 + n5, d_jil + n4 + n5, n6 - big6, d_out, d_joo + n4 + n5,
                                          d_jol + n4 + n5, d_got + n4 + n5, d_st + n4 + n5, max6, s);
         if (rc) return rc;
     }
     for (uint32_t k = n4 + n5 + n6 - big6; k < n4 + n5 + n6; k++) {
-        rc = hgpu_arith_decode_batch_dev(ctx, base + o_file, d_jio + k, d_jil + k, 1, base + o_out, d_joo + k, d_jol + k, d_got + k, d_st + k, jol[k], s);
+        rc = hgpu_arith_decode_batch_dev(ctx, d_file, d_jio + k, d_jil + k, 1, d_out, d_joo + k, d_jol + k, d_got + k, d_st + k, jol[k], s);
         if (rc == HGPU_ERR_NOMEM) nomem.push_back(k); else if (rc) return rc;
     }
     if (n1) {
         const uint32_t k0 = n4 + n5 + n6;
-        rc = hgpu_launch_gzip_inflate(ctx, base + o_file, d_jio + k0, d_jil + k0, n1, base + o_out, d_joo + k0, d_jol + k0, d_got + k0, d_st + k0, s);
+        rc = hgpu_launch_gzip_inflate(ctx, d_file, d_jio + k0, d_jil + k0, n1, d_out, d_joo + k0, d_jol + k0, d_got + k0, d_st + k0, s);
         if (rc) return rc;
     }
     std::vector<uint32_t> jgot(nj), crc(n);
     std::vector<int32_t> jst(nj);
-    if (out_span && hgpu_check(cudaMemcpyAsync(out + out_lo, base + o_out, out_span, cudaMemcpyDeviceToHost, s), "D2H")) return HGPU_ERR_CUDA;
-    if (nj) {
-        if (hgpu_check(cudaMemcpyAsync(jgot.data(), d_got, (size_t)nj * 4, cudaMemcpyDeviceToHost, s), "D2H")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(jst.data(), d_st, (size_t)nj * 4, cudaMemcpyDeviceToHost, s), "D2H")) return HGPU_ERR_CUDA;
-    }
-    if (hgpu_check(cudaMemcpyAsync(crc.data(), base + o_crc, (size_t)n * 4, cudaMemcpyDeviceToHost, s), "D2H")) return HGPU_ERR_CUDA;
+    if (hgpu_d2h(out + out_lo, d_out, out_span, s) || hgpu_d2h(jgot.data(), d_got, (size_t)nj * 4, s) ||
+        hgpu_d2h(jst.data(), d_st, (size_t)nj * 4, s) || hgpu_d2h(crc.data(), L.at(s_crc), (size_t)n * 4, s)) return HGPU_ERR_CUDA;
     if (hgpu_check(cudaStreamSynchronize(s), "sync")) return HGPU_ERR_CUDA;
 
     for (uint32_t k : nomem) jst[k] = HGPU_CRAM_ERR_DECODE;                    // never launched: its status word is stale
@@ -236,14 +217,5 @@ extern "C" int hgpu_cram_uncompress_blocks_host(hgpu_ctx *ctx, const uint8_t *fi
         const hgpu_cram_block *blocks, uint32_t n, uint8_t *out, const uint64_t *out_off,
         uint32_t *got_len, int32_t *status)
 {
-    // no C++ exception may cross the C ABI (a host buffer sized from a crafted file: std::bad_alloc)
-    try {
-        return cram_uncompress_impl(ctx, file, file_len, blocks, n, out, out_off, got_len, status);
-    } catch (const std::bad_alloc &) {
-        hgpu_set_error("out of host memory");
-        return HGPU_ERR_NOMEM;
-    } catch (...) {
-        hgpu_set_error("internal error");
-        return HGPU_ERR_CUDA;
-    }
+    return hgpu_abi_call([&] { return cram_uncompress_impl(ctx, file, file_len, blocks, n, out, out_off, got_len, status); });
 }

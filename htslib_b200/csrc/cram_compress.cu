@@ -10,23 +10,8 @@
 // LZMA (the device deflate writes BGZF members, not one zlib stream), FQZ (needs the slice's record lengths:
 // hgpu_fqz_encode_batch_host), TOK3 / TOKA (hgpu_tok3_encode_batch_host).
 #include "hgpu_internal.h"
-#include <new>
 #include <vector>
 #include <string.h>
-
-extern "C" {
-uint32_t hgpu_rans4x8_compress_bound(uint32_t size);
-int hgpu_rans4x8_encode_batch_dev(hgpu_ctx *, const uint8_t *, const uint64_t *, const uint32_t *, const uint32_t *, uint32_t, uint8_t *,
-                                  const uint64_t *, const uint32_t *, uint32_t *, int32_t *, void *);
-uint32_t hgpu_arith_compress_bound(uint32_t size, int order);
-int hgpu_arith_encode_batch_dev(hgpu_ctx *, const uint8_t *, const uint64_t *, const uint32_t *, const uint32_t *, uint32_t, uint8_t *,
-                                const uint64_t *, const uint32_t *, uint32_t *, int32_t *, uint32_t, void *);
-uint32_t hgpu_rans_nx16_compress_bound(uint32_t size, int order);
-int hgpu_rans_nx16_encode_batch_dev(hgpu_ctx *, const uint8_t *, const uint64_t *, const uint32_t *, const uint32_t *, uint32_t, uint8_t *,
-                                    const uint64_t *, const uint32_t *, uint32_t *, int32_t *, void *);
-int hgpu_cram_write_blocks_host(hgpu_ctx *ctx, const hgpu_cram_block *blocks, const uint8_t *const *payload, uint32_t n,
-                                uint8_t *out, uint64_t cap, uint64_t *out_off, uint64_t *out_len);
-}
 
 namespace {
 
@@ -87,37 +72,33 @@ int compress_impl(hgpu_ctx *ctx, const uint8_t *const *payload, const uint32_t *
         }
     }
     first[3] = pos;
-    const size_t o_in = 0, o_out = up16(in_off[n] + 64), o_jobs = o_out + up16(out_bytes + 64);
-    const size_t jb = up16((nc + 1) * 8);
-    const size_t total = o_jobs + 2 * jb + 5 * up16((nc + 1) * 4) + 1024;
-    int rc = hgpu_ensure_stage(ctx, total);
+    StageLayout L;
+    const auto s_in = L.seg(in_off[n] + 64), s_out = L.seg(out_bytes + 64), s_cin = L.seg((nc + 1) * 8), s_cout = L.seg((nc + 1) * 8),
+               s_len = L.seg((nc + 1) * 4), s_ord = L.seg((nc + 1) * 4), s_cap = L.seg((nc + 1) * 4), s_got = L.seg((nc + 1) * 4),
+               s_st = L.seg((nc + 1) * 4);
+    int rc = hgpu_stage_ensure(ctx, L);
     if (rc) return rc;
-    uint8_t *base = ctx->d_stage;
     cudaStream_t st = ctx->stream;
+    uint8_t *d_in = L.at(s_in), *d_out = L.at(s_out);
     for (uint32_t i = 0; i < n; i++)
-        if (payload_len[i] && hgpu_check(cudaMemcpyAsync(base + o_in + in_off[i], payload[i], payload_len[i], cudaMemcpyHostToDevice, st), "H2D")) return HGPU_ERR_CUDA;
-    uint64_t *d_cin = (uint64_t *)(base + o_jobs), *d_cout = (uint64_t *)(base + o_jobs + jb);
-    uint32_t *d_len = (uint32_t *)(base + o_jobs + 2 * jb), *d_ord = d_len + up16((nc + 1) * 4) / 4, *d_cap = d_ord + up16((nc + 1) * 4) / 4,
-             *d_got = d_cap + up16((nc + 1) * 4) / 4;
-    int32_t *d_st = (int32_t *)(d_got + up16((nc + 1) * 4) / 4);
+        if (hgpu_h2d(d_in + in_off[i], payload[i], payload_len[i], st)) return HGPU_ERR_CUDA;
+    uint64_t *d_cin = L.at<uint64_t>(s_cin), *d_cout = L.at<uint64_t>(s_cout);
+    uint32_t *d_len = L.at<uint32_t>(s_len), *d_ord = L.at<uint32_t>(s_ord), *d_cap = L.at<uint32_t>(s_cap), *d_got = L.at<uint32_t>(s_got);
+    int32_t *d_st = L.at<int32_t>(s_st);
     std::vector<uint32_t> got((size_t)nc + 1, 0);
     std::vector<int32_t> stt((size_t)nc + 1, 0);
     if (nc) {
-        if (hgpu_check(cudaMemcpyAsync(d_cin, c_in.data(), nc * 8, cudaMemcpyHostToDevice, st), "H2D") ||
-            hgpu_check(cudaMemcpyAsync(d_cout, c_out.data(), nc * 8, cudaMemcpyHostToDevice, st), "H2D") ||
-            hgpu_check(cudaMemcpyAsync(d_len, c_len.data(), nc * 4, cudaMemcpyHostToDevice, st), "H2D") ||
-            hgpu_check(cudaMemcpyAsync(d_ord, c_ord.data(), nc * 4, cudaMemcpyHostToDevice, st), "H2D") ||
-            hgpu_check(cudaMemcpyAsync(d_cap, c_cap.data(), nc * 4, cudaMemcpyHostToDevice, st), "H2D")) return HGPU_ERR_CUDA;
+        if (hgpu_h2d(d_cin, c_in.data(), nc * 8, st) || hgpu_h2d(d_cout, c_out.data(), nc * 8, st) || hgpu_h2d(d_len, c_len.data(), nc * 4, st) ||
+            hgpu_h2d(d_ord, c_ord.data(), nc * 4, st) || hgpu_h2d(d_cap, c_cap.data(), nc * 4, st)) return HGPU_ERR_CUDA;
         for (int c = 0; c < 3; c++) {
             const size_t f = first[c], m = first[c + 1] - first[c];
             if (!m) continue;
-            if (c == 0) rc = hgpu_rans4x8_encode_batch_dev(ctx, base + o_in, d_cin + f, d_len + f, d_ord + f, (uint32_t)m, base + o_out, d_cout + f, d_cap + f, d_got + f, d_st + f, st);
-            else if (c == 1) rc = hgpu_rans_nx16_encode_batch_dev(ctx, base + o_in, d_cin + f, d_len + f, d_ord + f, (uint32_t)m, base + o_out, d_cout + f, d_cap + f, d_got + f, d_st + f, st);
-            else rc = hgpu_arith_encode_batch_dev(ctx, base + o_in, d_cin + f, d_len + f, d_ord + f, (uint32_t)m, base + o_out, d_cout + f, d_cap + f, d_got + f, d_st + f, max_in, st);
+            if (c == 0) rc = hgpu_rans4x8_encode_batch_dev(ctx, d_in, d_cin + f, d_len + f, d_ord + f, (uint32_t)m, d_out, d_cout + f, d_cap + f, d_got + f, d_st + f, st);
+            else if (c == 1) rc = hgpu_rans_nx16_encode_batch_dev(ctx, d_in, d_cin + f, d_len + f, d_ord + f, (uint32_t)m, d_out, d_cout + f, d_cap + f, d_got + f, d_st + f, st);
+            else rc = hgpu_arith_encode_batch_dev(ctx, d_in, d_cin + f, d_len + f, d_ord + f, (uint32_t)m, d_out, d_cout + f, d_cap + f, d_got + f, d_st + f, max_in, st);
             if (rc) return rc;
         }
-        if (hgpu_check(cudaMemcpyAsync(got.data(), d_got, nc * 4, cudaMemcpyDeviceToHost, st), "D2H") ||
-            hgpu_check(cudaMemcpyAsync(stt.data(), d_st, nc * 4, cudaMemcpyDeviceToHost, st), "D2H") ||
+        if (hgpu_d2h(got.data(), d_got, nc * 4, st) || hgpu_d2h(stt.data(), d_st, nc * 4, st) ||
             hgpu_check(cudaStreamSynchronize(st), "cram compress")) return HGPU_ERR_CUDA;
     }
     // winners
@@ -139,7 +120,7 @@ int compress_impl(hgpu_ctx *ctx, const uint8_t *const *payload, const uint32_t *
         const Cand &c = cand[(size_t)best[i]];
         const size_t j = slot[(size_t)best[i]];
         comp[i].resize(got[j]);
-        if (hgpu_check(cudaMemcpyAsync(comp[i].data(), base + o_out + c_out[j], got[j], cudaMemcpyDeviceToHost, st), "D2H")) return HGPU_ERR_CUDA;
+        if (hgpu_d2h(comp[i].data(), d_out + c_out[j], got[j], st)) return HGPU_ERR_CUDA;
         blk[i].method = (uint8_t)(c.codec == 0 ? 4 : c.codec == 1 ? 5 : 6);   // the externalised method (cram_structs.h:219-230)
         blk[i].comp_size = got[j];
         pay[i] = comp[i].data();
@@ -155,7 +136,6 @@ extern "C" int hgpu_cram_compress_blocks_host(hgpu_ctx *ctx, const uint8_t *cons
         const uint32_t *method_mask, const int32_t *content_id, const uint8_t *content_type, uint32_t n,
         uint8_t *out, uint64_t cap, uint64_t *out_off, uint64_t *out_len, int32_t *chosen)
 {
-    try { return compress_impl(ctx, payload, payload_len, method_mask, content_id, content_type, n, out, cap, out_off, out_len, chosen); }
-    catch (const std::bad_alloc &) { hgpu_set_error("out of host memory"); return HGPU_ERR_NOMEM; }
-    catch (...) { hgpu_set_error("internal error"); return HGPU_ERR_NOMEM; }
+    return hgpu_abi_call([&] { return compress_impl(ctx, payload, payload_len, method_mask, content_id, content_type, n, out, cap, out_off, out_len, chosen); },
+                         HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
 }

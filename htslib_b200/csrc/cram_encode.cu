@@ -23,7 +23,7 @@ struct hgpu_ctx;
 #include "hgpu_internal.h"
 #endif
 #include "cram_encode.cuh"
-#include <new>
+#include "stage_layout.h"
 #include <map>
 #include <string>
 #include <vector>
@@ -31,16 +31,6 @@ struct hgpu_ctx;
 #include <string.h>
 
 using namespace cramenc;
-
-// (declared at file scope: inside the unnamed namespace they would get hidden visibility and drag the definitions with them)
-#ifndef HGPU_HOSTSIM
-extern "C" int hgpu_cram_compress_blocks_host(hgpu_ctx *ctx, const uint8_t *const *payload, const uint32_t *payload_len,
-        const uint32_t *method_mask, const int32_t *content_id, const uint8_t *content_type, uint32_t n,
-        uint8_t *out, uint64_t cap, uint64_t *out_off, uint64_t *out_len, int32_t *chosen);
-extern "C" int hgpu_tok3_encode_batch_host(hgpu_ctx *ctx, const uint8_t *in, const uint64_t *in_off, const uint32_t *in_len, uint32_t n,
-        uint8_t *out, const uint64_t *out_off, const uint32_t *out_cap, uint32_t *out_len, int32_t *status);
-#endif
-
 
 namespace {
 
@@ -195,8 +185,6 @@ __global__ void __launch_bounds__(128) cram_enc_write_kernel(EArgs A)
 }
 #endif
 
-inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, const hgpu_bam1_core *core, const uint8_t *data,
                 const uint64_t *data_off, uint64_t n, const hgpu_cram_refs *refs, uint32_t rps, int minor, uint8_t **out_file, uint64_t *out_len)
 {
@@ -249,42 +237,37 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
     std::vector<uint8_t> arena_h;
     const uint64_t data_bytes = n ? data_off[n] : 0;
     if (n) {
-        struct Seg { size_t off, bytes; };
-        size_t total = 0;
-        auto seg = [&](size_t bytes) { Seg s{total, bytes}; total += up256(bytes + 16); return s; };
-        const Seg s_ref = seg(ref_bytes), s_roff = seg(use_ref ? ((size_t)refs->n_ref + 1) * 8 : 0);
-        const Seg s_core = seg(n * 48), s_data = seg(data_bytes), s_doff = seg((n + 1) * 8), s_tl = seg(n * 4), s_cnt = seg(rows * rps * 4),
-                  s_tot = seg(rows * 4), s_base = seg(rows * 8), s_st = seg(n * 4);
+        StageLayout L(16);
+        const auto s_ref = L.seg(ref_bytes), s_roff = L.seg(use_ref ? ((size_t)refs->n_ref + 1) * 8 : 0);
+        const auto s_core = L.seg(n * 48), s_data = L.seg(data_bytes), s_doff = L.seg((n + 1) * 8), s_tl = L.seg(n * 4), s_cnt = L.seg(rows * rps * 4),
+                   s_tot = L.seg(rows * 4), s_base = L.seg(rows * 8), s_st = L.seg(n * 4);
         // every series byte comes from the record data, ITF8 at most 5 bytes per value: bound the arena before the scan
-        const size_t arena_cap = up256(2 * data_bytes + 200 * n + 4096);
-        const Seg s_arena = seg(arena_cap);
+        const size_t arena_cap = StageLayout::align(2 * data_bytes + 200 * n + 4096);
+        const auto s_arena = L.seg(arena_cap);
 #ifdef HGPU_HOSTSIM
         (void)ctx;
-        std::vector<uint8_t> image(total);
-        uint8_t *b0 = image.data();
-        memcpy(b0 + s_core.off, core, n * 48); memcpy(b0 + s_data.off, data, data_bytes); memcpy(b0 + s_doff.off, data_off, (n + 1) * 8);
-        memcpy(b0 + s_tl.off, tl.data(), n * 4);
-        if (use_ref) { memcpy(b0 + s_ref.off, refs->bases, ref_bytes); memcpy(b0 + s_roff.off, refs->off, ((size_t)refs->n_ref + 1) * 8); }
+        std::vector<uint8_t> image(L.total);
+        L.base = image.data();
+        memcpy(L.at(s_core), core, n * 48); memcpy(L.at(s_data), data, data_bytes); memcpy(L.at(s_doff), data_off, (n + 1) * 8);
+        memcpy(L.at(s_tl), tl.data(), n * 4);
+        if (use_ref) { memcpy(L.at(s_ref), refs->bases, ref_bytes); memcpy(L.at(s_roff), refs->off, ((size_t)refs->n_ref + 1) * 8); }
 #else
         if (!ctx) { hgpu_set_error("null context"); return HGPU_ERR_ARG; }
         if (cudaSetDevice(ctx->device) != cudaSuccess) return HGPU_ERR_CUDA;
-        int rc0 = hgpu_ensure_stage(ctx, total + 256);
+        int rc0 = hgpu_stage_ensure(ctx, L);
         if (rc0) return rc0;
-        uint8_t *b0 = ctx->d_stage;
         cudaStream_t st = ctx->stream;
-        if (hgpu_check(cudaMemcpyAsync(b0 + s_core.off, core, n * 48, cudaMemcpyHostToDevice, st), "H2D") ||
-            hgpu_check(cudaMemcpyAsync(b0 + s_data.off, data, data_bytes, cudaMemcpyHostToDevice, st), "H2D") ||
-            hgpu_check(cudaMemcpyAsync(b0 + s_doff.off, data_off, (n + 1) * 8, cudaMemcpyHostToDevice, st), "H2D") ||
-            hgpu_check(cudaMemcpyAsync(b0 + s_tl.off, tl.data(), n * 4, cudaMemcpyHostToDevice, st), "H2D")) return HGPU_ERR_CUDA;
-        if (use_ref && (hgpu_check(cudaMemcpyAsync(b0 + s_ref.off, refs->bases, ref_bytes, cudaMemcpyHostToDevice, st), "H2D") ||
-                        hgpu_check(cudaMemcpyAsync(b0 + s_roff.off, refs->off, ((size_t)refs->n_ref + 1) * 8, cudaMemcpyHostToDevice, st), "H2D"))) return HGPU_ERR_CUDA;
+        if (hgpu_h2d(L.at(s_core), core, n * 48, st) || hgpu_h2d(L.at(s_data), data, data_bytes, st) ||
+            hgpu_h2d(L.at(s_doff), data_off, (n + 1) * 8, st) || hgpu_h2d(L.at(s_tl), tl.data(), n * 4, st)) return HGPU_ERR_CUDA;
+        if (use_ref && (hgpu_h2d(L.at(s_ref), refs->bases, ref_bytes, st) ||
+                        hgpu_h2d(L.at(s_roff), refs->off, ((size_t)refs->n_ref + 1) * 8, st))) return HGPU_ERR_CUDA;
 #endif
         EArgs A;
-        A.core = reinterpret_cast<const Core *>(b0 + s_core.off); A.data = b0 + s_data.off; A.data_off = reinterpret_cast<const uint64_t *>(b0 + s_doff.off);
-        A.tl = reinterpret_cast<const int32_t *>(b0 + s_tl.off); A.n = n; A.rps = rps;
-        A.ref_bases = use_ref ? b0 + s_ref.off : nullptr; A.ref_off = reinterpret_cast<const uint64_t *>(b0 + s_roff.off); A.n_ref = use_ref ? refs->n_ref : 0;
-        A.cnt = reinterpret_cast<uint32_t *>(b0 + s_cnt.off); A.tot = reinterpret_cast<uint32_t *>(b0 + s_tot.off);
-        A.base = reinterpret_cast<const uint64_t *>(b0 + s_base.off); A.arena = b0 + s_arena.off; A.status = reinterpret_cast<int32_t *>(b0 + s_st.off);
+        A.core = L.at<Core>(s_core); A.data = L.at(s_data); A.data_off = L.at<uint64_t>(s_doff);
+        A.tl = L.at<int32_t>(s_tl); A.n = n; A.rps = rps;
+        A.ref_bases = use_ref ? L.at(s_ref) : nullptr; A.ref_off = L.at<uint64_t>(s_roff); A.n_ref = use_ref ? refs->n_ref : 0;
+        A.cnt = L.at<uint32_t>(s_cnt); A.tot = L.at<uint32_t>(s_tot);
+        A.base = L.at<uint64_t>(s_base); A.arena = L.at(s_arena); A.status = L.at<int32_t>(s_st);
 #ifdef HGPU_HOSTSIM
         for (uint64_t g = 0; g < n; g++) count_body(A, g);
         for (size_t row = 0; row < rows; row++) {
@@ -301,8 +284,7 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         cram_enc_scan_kernel<<<(unsigned)((rows + 3) / 4), 128, 0, st>>>(A, (uint32_t)rows);
         hgpu_count_launch(2);
         if (hgpu_check(cudaGetLastError(), "cram encode launch")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(tot.data(), A.tot, rows * 4, cudaMemcpyDeviceToHost, st), "D2H") ||
-            hgpu_check(cudaMemcpyAsync(status.data(), A.status, n * 4, cudaMemcpyDeviceToHost, st), "D2H") ||
+        if (hgpu_d2h(tot.data(), A.tot, rows * 4, st) || hgpu_d2h(status.data(), A.status, n * 4, st) ||
             hgpu_check(cudaStreamSynchronize(st), "cram encode count")) return HGPU_ERR_CUDA;
 #endif
         for (uint64_t g = 0; g < n; g++)
@@ -316,15 +298,15 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         if (at > arena_cap) { hgpu_set_error("cram encode: series arena bound exceeded"); return HGPU_ERR_NOMEM; }
         arena_h.resize(at + 16);
 #ifdef HGPU_HOSTSIM
-        memcpy(b0 + s_base.off, base.data(), rows * 8);
+        memcpy(L.at(s_base), base.data(), rows * 8);
         for (uint64_t g = 0; g < n; g++) write_body(A, g);
         memcpy(arena_h.data(), A.arena, at);
 #else
-        if (hgpu_check(cudaMemcpyAsync(b0 + s_base.off, base.data(), rows * 8, cudaMemcpyHostToDevice, st), "H2D")) return HGPU_ERR_CUDA;
+        if (hgpu_h2d(L.at(s_base), base.data(), rows * 8, st)) return HGPU_ERR_CUDA;
         cram_enc_write_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A);
         hgpu_count_launch();
         if (hgpu_check(cudaGetLastError(), "cram encode write launch")) return HGPU_ERR_CUDA;
-        if (at && hgpu_check(cudaMemcpyAsync(arena_h.data(), A.arena, at, cudaMemcpyDeviceToHost, st), "D2H")) return HGPU_ERR_CUDA;
+        if (hgpu_d2h(arena_h.data(), A.arena, at, st)) return HGPU_ERR_CUDA;
         if (hgpu_check(cudaStreamSynchronize(st), "cram encode write")) return HGPU_ERR_CUDA;
 #endif
     }
@@ -466,8 +448,7 @@ extern "C" int hgpu_cram_encode_records_host(hgpu_ctx *ctx, const char *header_t
         const uint8_t *data, const uint64_t *data_off, uint64_t n, const hgpu_cram_refs *refs, uint32_t records_per_slice, int minor_version,
         uint8_t **out_file, uint64_t *out_len)
 {
-    try { return encode_impl(ctx, header_text, header_len, core, data, data_off, n, refs, records_per_slice, minor_version, out_file, out_len); }
-    catch (const std::bad_alloc &) { hgpu_set_error("out of host memory"); return HGPU_ERR_NOMEM; }
-    catch (...) { hgpu_set_error("internal error"); return HGPU_ERR_NOMEM; }
+    return hgpu_abi_call([&] { return encode_impl(ctx, header_text, header_len, core, data, data_off, n, refs, records_per_slice, minor_version, out_file, out_len); },
+                         HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
 }
 #endif

@@ -217,17 +217,8 @@ static long hgpu_cram_parse_compression_header_impl(const uint8_t *hdr, uint32_t
     return (long)out.size();
 }
 
-// no C++ exception may cross the C ABI (host buffers are sized from untrusted input: std::bad_alloc)
 extern "C" long hgpu_cram_parse_compression_header(const uint8_t *hdr, uint32_t len, int major_version,
         hgpu_cram_series *series, long cap, char *text, size_t text_cap)
 {
-    try {
-        return hgpu_cram_parse_compression_header_impl(hdr, len, major_version, series, cap, text, text_cap);
-    } catch (const std::bad_alloc &) {
-        hgpu_set_error("out of host memory");
-        return -1;
-    } catch (...) {
-        hgpu_set_error("internal error");
-        return -1;
-    }
+    return hgpu_abi_call([&] { return hgpu_cram_parse_compression_header_impl(hdr, len, major_version, series, cap, text, text_cap); }, -1, -1);
 }

@@ -24,7 +24,7 @@ struct hgpu_ctx;
 #include "hgpu_internal.h"
 #endif
 #include "cram_records.cuh"
-#include <new>
+#include "stage_layout.h"
 #include <map>
 #include <string>
 #include <vector>
@@ -36,8 +36,8 @@ using namespace cramrec;
 
 #ifdef HGPU_HOSTSIM
 #define hgpu_cram_records_free hostsim_cram_records_free
-#endif
 extern "C" void hgpu_cram_records_free(hgpu_cram_records *r);
+#endif
 static_assert(sizeof(BamCore) == 48 && sizeof(hgpu_bam1_core) == 48, "bam1_core_t mirror");
 
 namespace {
@@ -521,8 +521,6 @@ __global__ void __launch_bounds__(128) cram_bam_fill_kernel(Args A)
 }
 #endif
 
-inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n_blocks,
                 const uint8_t *udata, const uint64_t *udata_off, const hgpu_cram_refs *refs, const char *name_prefix, int decode_md,
                 hgpu_cram_records *out, hgpu_cram_records_dev *dev = nullptr)
@@ -544,7 +542,8 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
     std::vector<uint8_t> slice_ok;                         // 0: flagged before launch (table not usable)
     int32_t cur_table = -1;
     bool have_header = false;
-    uint64_t n_records = 0, scratch_bytes = 0;
+    uint64_t n_records = 0;
+    StageLayout scratch;                                   // per-slice arenas inside the scratch region
     uint64_t udata_end = 0;
     for (uint32_t i = 0; i < n_blocks; i++) udata_end = std::max<uint64_t>(udata_end, udata_off[i] + blocks[i].uncomp_size);
     const uint32_t prefix_len = name_prefix ? (uint32_t)strlen(name_prefix) : 0;
@@ -631,10 +630,10 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
             S.rec0 = n_records;
             n_records += nr;
             if (ok) {
-                S.name_off = scratch_bytes; S.name_cap = (uint32_t)name_cap; scratch_bytes += up256(name_cap);
-                S.seq_off = scratch_bytes; S.seq_cap = (uint32_t)seq_cap; scratch_bytes += up256(2 * seq_cap);
-                S.aux_off = scratch_bytes; S.aux_cap = (uint32_t)aux_cap; scratch_bytes += up256(aux_cap);
-                S.cig_off = scratch_bytes; S.cig_cap = (uint32_t)cig_cap; scratch_bytes += up256(4 * cig_cap);
+                S.name_off = scratch.seg(name_cap).off; S.name_cap = (uint32_t)name_cap;
+                S.seq_off = scratch.seg(2 * seq_cap).off; S.seq_cap = (uint32_t)seq_cap;
+                S.aux_off = scratch.seg(aux_cap).off; S.aux_cap = (uint32_t)aux_cap;
+                S.cig_off = scratch.seg(4 * cig_cap).off; S.cig_cap = (uint32_t)cig_cap;
             }
             slices.push_back(S);
             slice_ok.push_back(ok ? 1 : 0);
@@ -670,32 +669,28 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
 
     // one device image: [udata | refs | tables | pools | slices | ext | cur | scratch | recs | per-record arrays]
     const uint64_t ref_bytes = refs && refs->bases ? refs->off[nref] : 0;
-    struct Seg { size_t off, bytes; };
-    size_t total = 0;
-    auto seg = [&](size_t bytes) { Seg s{total, bytes}; total += up256(bytes + 16); return s; };
-    const Seg s_udata = seg(udata_end), s_ref = seg(ref_bytes), s_refoff = seg((size_t)(nref + 2) * 8), s_sqlen = seg((size_t)(nref + 1) * 8),
-              s_tab = seg(B.tables.size() * sizeof(Table)), s_cp = seg(B.cpool.size() * sizeof(Codec)), s_hp = seg(B.hpool.size() * sizeof(HuffCode)),
-              s_tk = seg(B.tagkeys.size() * 4), s_tl = seg(B.tlidx.size() * 4), s_td = seg(B.td.size() + 8), s_sl = seg((size_t)ns * sizeof(Slice)),
-              s_ext = seg(ext.size() * sizeof(Ext)), s_cur = seg(ext.size() * 4), s_rgn = seg(rg_names.size()), s_rgo = seg(rg_off.size() * 4),
-              s_rgl = seg(rg_len.size() * 4), s_pre = seg(prefix_len + 1), s_scr = seg(scratch_bytes), s_recs = seg(n_records * sizeof(Rec)),
-              s_rsl = seg(n_records * 4), s_loff = seg(n_records * 8), s_sby = seg((size_t)ns * 8), s_sst = seg((size_t)ns * 4), s_sbase = seg((size_t)(ns + 1) * 8),
-              s_core = seg(n_records * sizeof(BamCore)), s_doff = seg((n_records + 1) * 8), s_rst = seg(n_records * 4);
+    StageLayout L(16);
+    const auto s_udata = L.seg(udata_end), s_ref = L.seg(ref_bytes), s_refoff = L.seg((size_t)(nref + 2) * 8), s_sqlen = L.seg((size_t)(nref + 1) * 8),
+               s_tab = L.seg(B.tables.size() * sizeof(Table)), s_cp = L.seg(B.cpool.size() * sizeof(Codec)), s_hp = L.seg(B.hpool.size() * sizeof(HuffCode)),
+               s_tk = L.seg(B.tagkeys.size() * 4), s_tl = L.seg(B.tlidx.size() * 4), s_td = L.seg(B.td.size() + 8), s_sl = L.seg((size_t)ns * sizeof(Slice)),
+               s_ext = L.seg(ext.size() * sizeof(Ext)), s_cur = L.seg(ext.size() * 4), s_rgn = L.seg(rg_names.size()), s_rgo = L.seg(rg_off.size() * 4),
+               s_rgl = L.seg(rg_len.size() * 4), s_pre = L.seg(prefix_len + 1), s_scr = L.seg(scratch.total), s_recs = L.seg(n_records * sizeof(Rec)),
+               s_rsl = L.seg(n_records * 4), s_loff = L.seg(n_records * 8), s_sby = L.seg((size_t)ns * 8), s_sst = L.seg((size_t)ns * 4), s_sbase = L.seg((size_t)(ns + 1) * 8),
+               s_core = L.seg(n_records * sizeof(BamCore)), s_doff = L.seg((n_records + 1) * 8), s_rst = L.seg(n_records * 4);
     for (uint32_t s = 0; s < ns; s++) if (!slice_ok[s]) slices[s].table = -1;      // the kernel skips these
 
 #ifdef HGPU_HOSTSIM
     (void)ctx;
-    std::vector<uint8_t> image(total);
-    uint8_t *base = image.data();
-#define UP(seg, src, n) do { if (n) memcpy(base + (seg).off, (src), (n)); } while (0)
+    std::vector<uint8_t> image(L.total);
+    L.base = image.data();
+#define UP(seg, src, n) do { if (n) memcpy(L.at(seg), (src), (n)); } while (0)
 #else
     if (!ctx) { hgpu_set_error("null context"); return HGPU_ERR_ARG; }
     if (cudaSetDevice(ctx->device) != cudaSuccess) return HGPU_ERR_CUDA;
-    int rc0 = hgpu_ensure_stage(ctx, total + 256);
+    int rc0 = hgpu_stage_ensure(ctx, L);
     if (rc0) return rc0;
-    uint8_t *base = ctx->d_stage;
     cudaStream_t st = ctx->stream;
-    bool up_fail = false;
-#define UP(seg, src, n) do { if ((n) && cudaMemcpyAsync(base + (seg).off, (src), (n), cudaMemcpyHostToDevice, st) != cudaSuccess) up_fail = true; } while (0)
+#define UP(seg, src, n) do { if (!rc0) rc0 = hgpu_h2d(L.at(seg), (src), (n), st); } while (0)
 #endif
     std::vector<uint64_t> refoff((size_t)nref + 2, 0);
     if (ref_bytes) for (int32_t k = 0; k <= nref; k++) refoff[(size_t)k] = refs->off[k];
@@ -718,34 +713,33 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
 
     Args A;
     memset(&A, 0, sizeof A);
-    A.P.tables = reinterpret_cast<const Table *>(base + s_tab.off); A.P.cpool = reinterpret_cast<const Codec *>(base + s_cp.off);
-    A.P.hpool = reinterpret_cast<const HuffCode *>(base + s_hp.off); A.P.tagkeys = reinterpret_cast<const uint32_t *>(base + s_tk.off);
-    A.P.tlidx = reinterpret_cast<const uint32_t *>(base + s_tl.off); A.P.td = base + s_td.off;
-    A.P.ext = reinterpret_cast<const Ext *>(base + s_ext.off); A.P.cur = reinterpret_cast<uint32_t *>(base + s_cur.off); A.P.udata = base + s_udata.off;
-    A.slices = reinterpret_cast<const Slice *>(base + s_sl.off); A.n_slices = ns;
-    A.R.bases = ref_bytes ? base + s_ref.off : nullptr; A.R.off = reinterpret_cast<const uint64_t *>(base + s_refoff.off);
-    A.R.sq_len = reinterpret_cast<const int64_t *>(base + s_sqlen.off); A.R.n_ref = nref;
-    A.scratch = base + s_scr.off; A.recs = reinterpret_cast<Rec *>(base + s_recs.off); A.rec_slice = reinterpret_cast<uint32_t *>(base + s_rsl.off);
-    A.local_off = reinterpret_cast<uint64_t *>(base + s_loff.off); A.slice_bytes = reinterpret_cast<uint64_t *>(base + s_sby.off);
-    A.slice_status = reinterpret_cast<int32_t *>(base + s_sst.off);
-    A.rg_names = base + s_rgn.off; A.rg_off = reinterpret_cast<const uint32_t *>(base + s_rgo.off); A.rg_len = reinterpret_cast<const uint32_t *>(base + s_rgl.off);
+    A.P.tables = L.at<Table>(s_tab); A.P.cpool = L.at<Codec>(s_cp);
+    A.P.hpool = L.at<HuffCode>(s_hp); A.P.tagkeys = L.at<uint32_t>(s_tk);
+    A.P.tlidx = L.at<uint32_t>(s_tl); A.P.td = L.at(s_td);
+    A.P.ext = L.at<Ext>(s_ext); A.P.cur = L.at<uint32_t>(s_cur); A.P.udata = L.at(s_udata);
+    A.slices = L.at<Slice>(s_sl); A.n_slices = ns;
+    A.R.bases = ref_bytes ? L.at(s_ref) : nullptr; A.R.off = L.at<uint64_t>(s_refoff);
+    A.R.sq_len = L.at<int64_t>(s_sqlen); A.R.n_ref = nref;
+    A.scratch = L.at(s_scr); A.recs = L.at<Rec>(s_recs); A.rec_slice = L.at<uint32_t>(s_rsl);
+    A.local_off = L.at<uint64_t>(s_loff); A.slice_bytes = L.at<uint64_t>(s_sby);
+    A.slice_status = L.at<int32_t>(s_sst);
+    A.rg_names = L.at(s_rgn); A.rg_off = L.at<uint32_t>(s_rgo); A.rg_len = L.at<uint32_t>(s_rgl);
     A.nrg = (int32_t)H.rg.size(); A.unknown_rg = H.unknown_rg;
-    A.prefix = base + s_pre.off; A.prefix_len = prefix_len;
+    A.prefix = L.at(s_pre); A.prefix_len = prefix_len;
     A.decode_md = decode_md;
-    A.slice_base = reinterpret_cast<const uint64_t *>(base + s_sbase.off);
-    A.core = reinterpret_cast<BamCore *>(base + s_core.off); A.data_off = reinterpret_cast<uint64_t *>(base + s_doff.off);
-    A.rec_status = reinterpret_cast<int32_t *>(base + s_rst.off); A.n_records = n_records;
+    A.slice_base = L.at<uint64_t>(s_sbase);
+    A.core = L.at<BamCore>(s_core); A.data_off = L.at<uint64_t>(s_doff);
+    A.rec_status = L.at<int32_t>(s_rst); A.n_records = n_records;
 
     std::vector<uint64_t> sbytes(ns), sbase((size_t)ns + 1, 0);
     std::vector<int32_t> sstat(ns);
 #ifdef HGPU_HOSTSIM
-    memset(base + s_cur.off, 0, ext.size() * 4);
+    memset(L.at(s_cur), 0, ext.size() * 4);
     for (uint32_t s = 0; s < ns; s++) slice_body<HostW>(A, s, 0, 1);
     memcpy(sbytes.data(), A.slice_bytes, (size_t)ns * 8);
     memcpy(sstat.data(), A.slice_status, (size_t)ns * 4);
 #else
-    if (cudaMemsetAsync(base + s_cur.off, 0, ext.size() * 4 + 4, st) != cudaSuccess) up_fail = true;
-    if (up_fail) { hgpu_set_error("cram records: upload failed: %s", cudaGetErrorString(cudaGetLastError())); return HGPU_ERR_CUDA; }
+    if (rc0 || (rc0 = hgpu_memset(L.at(s_cur), 0, ext.size() * 4 + 4, st))) return rc0;
     struct Events {                                  // destroyed on every return path
         cudaEvent_t e[4]; int n = 0;
         bool make() { for (; n < 4; n++) if (cudaEventCreate(&e[n]) != cudaSuccess) return false; return true; }
@@ -758,8 +752,7 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
     cudaEventRecord(ev[1], st);
     hgpu_count_launch();
     if (hgpu_check(cudaGetLastError(), "cram slice decode launch")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(sbytes.data(), A.slice_bytes, (size_t)ns * 8, cudaMemcpyDeviceToHost, st), "D2H")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(sstat.data(), A.slice_status, (size_t)ns * 4, cudaMemcpyDeviceToHost, st), "D2H")) return HGPU_ERR_CUDA;
+    if (hgpu_d2h(sbytes.data(), A.slice_bytes, (size_t)ns * 8, st) || hgpu_d2h(sstat.data(), A.slice_status, (size_t)ns * 4, st)) return HGPU_ERR_CUDA;
     if (hgpu_check(cudaStreamSynchronize(st), "cram slice decode")) return HGPU_ERR_CUDA;
 #endif
     for (uint32_t s = 0; s < ns; s++) { if (sstat[s] != 0) sbytes[s] = 0; sbase[s + 1] = sbase[s] + sbytes[s]; }
@@ -770,7 +763,7 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
     for (uint32_t s = 0; s < ns; s++) out->slice_status[s] = sstat[s] == ERR_SPACE ? HGPU_CRAM_ERR_SPACE : sstat[s] == ERR_NOREF ? HGPU_CRAM_ERR_NOREF : sstat[s];
 
 #ifdef HGPU_HOSTSIM
-    memcpy(base + s_sbase.off, sbase.data(), sbase.size() * 8);
+    memcpy(L.at(s_sbase), sbase.data(), sbase.size() * 8);
     std::vector<uint8_t> dbuf(data_bytes + 16);
     A.data = dbuf.data();
     for (uint64_t g = 0; g < n_records; g++) fill_body<HostW>(A, g);
@@ -783,7 +776,7 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
     int rc1 = hgpu_ensure_mrec(ctx, data_bytes + 256);            // (not d_bam: hgpu_sam_format_dev / hgpu_bam_pack_dev scan there)
     if (rc1) { hgpu_cram_records_free(out); return rc1; }
     A.data = ctx->d_mrec;
-    if (hgpu_check(cudaMemcpyAsync(base + s_sbase.off, sbase.data(), sbase.size() * 8, cudaMemcpyHostToDevice, st), "H2D")) return HGPU_ERR_CUDA;
+    if (hgpu_h2d(L.at(s_sbase), sbase.data(), sbase.size() * 8, st)) return HGPU_ERR_CUDA;
     cudaEventRecord(ev[2], st);
     cram_bam_fill_kernel<<<(unsigned)((n_records + 3) / 4), 128, 0, st>>>(A);
     cudaEventRecord(ev[3], st);
@@ -793,10 +786,8 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
         dev->n_records = n_records; dev->data_bytes = data_bytes;
         dev->d_core = reinterpret_cast<hgpu_bam1_core *>(A.core); dev->d_data = A.data; dev->d_data_off = A.data_off; dev->d_rec_status = A.rec_status;
     } else {
-        if (hgpu_check(cudaMemcpyAsync(out->core, A.core, n_records * sizeof(BamCore), cudaMemcpyDeviceToHost, st), "D2H")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(out->data_off, A.data_off, (n_records + 1) * 8, cudaMemcpyDeviceToHost, st), "D2H")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(out->rec_status, A.rec_status, n_records * 4, cudaMemcpyDeviceToHost, st), "D2H")) return HGPU_ERR_CUDA;
-        if (data_bytes && hgpu_check(cudaMemcpyAsync(out->data, A.data, data_bytes, cudaMemcpyDeviceToHost, st), "D2H")) return HGPU_ERR_CUDA;
+        if (hgpu_d2h(out->core, A.core, n_records * sizeof(BamCore), st) || hgpu_d2h(out->data_off, A.data_off, (n_records + 1) * 8, st) ||
+            hgpu_d2h(out->rec_status, A.rec_status, n_records * 4, st) || hgpu_d2h(out->data, A.data, data_bytes, st)) return HGPU_ERR_CUDA;
     }
     if (hgpu_check(cudaStreamSynchronize(st), "cram bam fill")) return HGPU_ERR_CUDA;
     cudaEventElapsedTime(&g_last_ms[0], ev[0], ev[1]);
@@ -823,10 +814,6 @@ extern "C" int hostsim_cram_decode_records(const uint8_t *file, uint64_t file_le
     catch (...) { hgpu_set_error("internal error"); return HGPU_ERR_NOMEM; }
 }
 #else
-extern "C" long hgpu_cram_scan_blocks(const uint8_t *file, uint64_t len, hgpu_cram_block *blocks, long cap, int *major, int *minor);
-extern "C" int hgpu_cram_uncompress_blocks_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n,
-                                                 uint8_t *out, const uint64_t *out_off, uint32_t *got_len, int32_t *status);
-
 // scan + cram_uncompress_block for every block + record decode: a CRAM file image in, bam1_t records out
 static int decode_file_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_refs *refs, const char *name_prefix,
                             int decode_md, hgpu_cram_records *out)
@@ -855,9 +842,8 @@ extern "C" int hgpu_cram_decode_records_dev(hgpu_ctx *ctx, const uint8_t *file, 
         hgpu_cram_records *out, hgpu_cram_records_dev *dev)
 {
     if (!dev) { hgpu_set_error("cram records: null argument"); return HGPU_ERR_ARG; }
-    try { return decode_impl(ctx, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md, out, dev); }
-    catch (const std::bad_alloc &) { hgpu_set_error("out of host memory"); return HGPU_ERR_NOMEM; }
-    catch (...) { hgpu_set_error("internal error"); return HGPU_ERR_NOMEM; }
+    return hgpu_abi_call([&] { return decode_impl(ctx, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md, out, dev); },
+                         HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
 }
 
 extern "C" void hgpu_cram_records_last_ms(float *slice_decode_ms, float *bam_fill_ms)
@@ -869,16 +855,13 @@ extern "C" void hgpu_cram_records_last_ms(float *slice_decode_ms, float *bam_fil
 extern "C" int hgpu_cram_decode_file_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_refs *refs,
                                           const char *name_prefix, int decode_md, hgpu_cram_records *out)
 {
-    try { return decode_file_impl(ctx, file, file_len, refs, name_prefix, decode_md, out); }
-    catch (const std::bad_alloc &) { hgpu_set_error("out of host memory"); return HGPU_ERR_NOMEM; }
-    catch (...) { hgpu_set_error("internal error"); return HGPU_ERR_NOMEM; }
+    return hgpu_abi_call([&] { return decode_file_impl(ctx, file, file_len, refs, name_prefix, decode_md, out); }, HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
 }
 
 extern "C" int hgpu_cram_decode_records_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n_blocks,
         const uint8_t *udata, const uint64_t *udata_off, const hgpu_cram_refs *refs, const char *name_prefix, int decode_md, hgpu_cram_records *out)
 {
-    try { return decode_impl(ctx, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md, out); }
-    catch (const std::bad_alloc &) { hgpu_set_error("out of host memory"); return HGPU_ERR_NOMEM; }
-    catch (...) { hgpu_set_error("internal error"); return HGPU_ERR_NOMEM; }
+    return hgpu_abi_call([&] { return decode_impl(ctx, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md, out); },
+                         HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
 }
 #endif

@@ -145,16 +145,14 @@ extern "C" int hgpu_cram_write_blocks_host(hgpu_ctx *ctx, const hgpu_cram_block 
         p += (uint64_t)k + dl + 4;
     }
     // ---- one CRC launch over the image
-    auto up = [](uint64_t x) { return (x + 255) & ~(uint64_t)255; };
-    const uint64_t o_img = 0, o_coff = up(p + 8), o_clen = o_coff + up((uint64_t)n * 8), o_crc = o_clen + up((uint64_t)n * 4), total = o_crc + up((uint64_t)n * 4);
-    int rc = hgpu_ensure_stage(ctx, total + 256);
+    StageLayout L;
+    const auto s_img = L.seg(p + 8), s_coff = L.seg((size_t)n * 8), s_clen = L.seg((size_t)n * 4), s_crc = L.seg((size_t)n * 4);
+    int rc = hgpu_stage_ensure(ctx, L);
     cudaStream_t s = ctx->stream;
-    uint8_t *base = ctx->d_stage;
-    if (!rc && (hgpu_check(cudaMemcpyAsync(base + o_img, out, p, cudaMemcpyHostToDevice, s), "H2D") ||
-                hgpu_check(cudaMemcpyAsync(base + o_coff, coff, (size_t)n * 8, cudaMemcpyHostToDevice, s), "H2D") ||
-                hgpu_check(cudaMemcpyAsync(base + o_clen, clen, (size_t)n * 4, cudaMemcpyHostToDevice, s), "H2D"))) rc = HGPU_ERR_CUDA;
-    if (!rc) rc = hgpu_launch_crc32_batch(ctx, base + o_img, (const uint64_t *)(base + o_coff), (const uint32_t *)(base + o_clen), n, (uint32_t *)(base + o_crc), s);
-    if (!rc && (hgpu_check(cudaMemcpyAsync(crc, base + o_crc, (size_t)n * 4, cudaMemcpyDeviceToHost, s), "D2H") || hgpu_check(cudaStreamSynchronize(s), "sync"))) rc = HGPU_ERR_CUDA;
+    if (!rc && (hgpu_h2d(L.at(s_img), out, p, s) || hgpu_h2d(L.at(s_coff), coff, (size_t)n * 8, s) ||
+                hgpu_h2d(L.at(s_clen), clen, (size_t)n * 4, s))) rc = HGPU_ERR_CUDA;
+    if (!rc) rc = hgpu_launch_crc32_batch(ctx, L.at(s_img), L.at<uint64_t>(s_coff), L.at<uint32_t>(s_clen), n, L.at<uint32_t>(s_crc), s);
+    if (!rc && (hgpu_d2h(crc, L.at(s_crc), (size_t)n * 4, s) || hgpu_check(cudaStreamSynchronize(s), "sync"))) rc = HGPU_ERR_CUDA;
     if (!rc) for (uint32_t i = 0; i < n; i++) {
         uint8_t *q = out + coff[i] + clen[i];
         q[0] = (uint8_t)crc[i]; q[1] = (uint8_t)(crc[i] >> 8); q[2] = (uint8_t)(crc[i] >> 16); q[3] = (uint8_t)(crc[i] >> 24);

@@ -246,7 +246,9 @@ static int hgpu_fqz_encode_batch_host_impl(hgpu_ctx *ctx, const uint8_t *in, con
     // ---- host: parameters of every stream (fqz_pick_parameters :736-924 without the selector search)
     std::vector<EncStream> streams(n);
     std::vector<EncParam> params(n);
-    uint64_t in_end = 0, out_end = 0, rec_end = 0, model_words = 0;
+    uint64_t model_words = 0;
+    const uint64_t in_end = hgpu_slots_end(in_off, in_len, n), out_end = hgpu_slots_end(out_off, out_cap, n),
+                   rec_end = hgpu_slots_end(rec_off, nrec, n);
     for (uint32_t s = 0; s < n; s++) {
         EncStream &S = streams[s];
         EncParam &P = params[s];
@@ -254,9 +256,6 @@ static int hgpu_fqz_encode_batch_host_impl(hgpu_ctx *ctx, const uint8_t *in, con
         S.in_off = in_off[s]; S.in_len = in_len[s]; S.out_off = out_off[s]; S.out_cap = out_cap[s];
         S.rec_off = rec_off[s]; S.nrec = nrec[s];
         S.host_status = HGPU_FQZ_ERR;
-        if (in_off[s] + in_len[s] > in_end) in_end = in_off[s] + in_len[s];
-        if (out_off[s] + out_cap[s] > out_end) out_end = out_off[s] + out_cap[s];
-        if (rec_off[s] + nrec[s] > rec_end) rec_end = rec_off[s] + nrec[s];
         const uint8_t *q = in + in_off[s];
         const uint32_t *L = rec_len + rec_off[s];
         const uint32_t size = in_len[s];
@@ -326,50 +325,39 @@ static int hgpu_fqz_encode_batch_host_impl(hgpu_ctx *ctx, const uint8_t *in, con
         S.host_status = HGPU_OK;
     }
 
-    auto up = [](uint64_t x) { return (x + 255) & ~(uint64_t)255; };
-    const uint64_t o_in = 0, o_out = o_in + up(in_end + 8), o_rec = o_out + up(out_end + 8), o_streams = o_rec + up(rec_end * 4 + 8),
-                   o_params = o_streams + up((uint64_t)n * sizeof(EncStream)), o_olen = o_params + up((uint64_t)n * sizeof(EncParam)),
-                   o_st = o_olen + up((uint64_t)n * 4), o_models = o_st + up((uint64_t)n * 4), total = o_models + up(model_words * 4 + 16);
-    int rc = hgpu_ensure_stage(ctx, total + 256);
+    StageLayout L;
+    const auto s_in = L.seg(in_end + 8), s_out = L.seg(out_end + 8), s_rec = L.seg(rec_end * 4 + 8), s_streams = L.seg((size_t)n * sizeof(EncStream)),
+               s_params = L.seg((size_t)n * sizeof(EncParam)), s_olen = L.seg((size_t)n * 4), s_st = L.seg((size_t)n * 4),
+               s_models = L.seg(model_words * 4 + 16);
+    int rc = hgpu_stage_ensure(ctx, L);
     if (rc) return rc;
-    uint8_t *base = ctx->d_stage;
     cudaStream_t st = ctx->stream;
-    if (hgpu_check(cudaMemcpyAsync(base + o_in, in, in_end, cudaMemcpyHostToDevice, st), "H2D")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(base + o_out, out, out_end, cudaMemcpyHostToDevice, st), "H2D")) return HGPU_ERR_CUDA;   // the headers
-    if (hgpu_check(cudaMemcpyAsync(base + o_rec, rec_len, rec_end * 4, cudaMemcpyHostToDevice, st), "H2D")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(base + o_streams, streams.data(), (size_t)n * sizeof(EncStream), cudaMemcpyHostToDevice, st), "H2D")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(base + o_params, params.data(), (size_t)n * sizeof(EncParam), cudaMemcpyHostToDevice, st), "H2D")) return HGPU_ERR_CUDA;
+    const EncStream *d_streams = L.at<EncStream>(s_streams);
+    const EncParam *d_params = L.at<EncParam>(s_params);
+    if (hgpu_h2d(L.at(s_in), in, in_end, st) || hgpu_h2d(L.at(s_out), out, out_end, st) /* the headers */ ||
+        hgpu_h2d(L.at(s_rec), rec_len, rec_end * 4, st) || hgpu_h2d(L.at(s_streams), streams.data(), (size_t)n * sizeof(EncStream), st) ||
+        hgpu_h2d(L.at(s_params), params.data(), (size_t)n * sizeof(EncParam), st)) return HGPU_ERR_CUDA;
     for (uint32_t first = 0; first < n; first += 65535u) {
         const uint32_t cnt = n - first < 65535u ? n - first : 65535u;
-        fqz_enc_init_models_kernel<<<dim3(64, cnt), 256, 0, st>>>((const EncStream *)(base + o_streams) + first,
-                                                                   (const EncParam *)(base + o_params) + first, (uint32_t *)(base + o_models));
+        fqz_enc_init_models_kernel<<<dim3(64, cnt), 256, 0, st>>>(d_streams + first, d_params + first, L.at<uint32_t>(s_models));
         if (hgpu_check(cudaGetLastError(), "fqz_enc_init_models_kernel")) return HGPU_ERR_CUDA;
         hgpu_count_launch();
     }
-    fqz_encode_kernel<<<(n + 31) / 32, 32, 0, st>>>((const EncStream *)(base + o_streams), (const EncParam *)(base + o_params), 0, n,
-                                                   base + o_in, (const uint32_t *)(base + o_rec), (uint32_t *)(base + o_models),
-                                                   base + o_out, (uint32_t *)(base + o_olen), (int32_t *)(base + o_st));
+    fqz_encode_kernel<<<(n + 31) / 32, 32, 0, st>>>(d_streams, d_params, 0, n, L.at(s_in), L.at<uint32_t>(s_rec), L.at<uint32_t>(s_models),
+                                                   L.at(s_out), L.at<uint32_t>(s_olen), L.at<int32_t>(s_st));
     if (hgpu_check(cudaGetLastError(), "fqz_encode_kernel")) return HGPU_ERR_CUDA;
     hgpu_count_launch();
-    if (hgpu_check(cudaMemcpyAsync(out_len, base + o_olen, (size_t)n * 4, cudaMemcpyDeviceToHost, st), "D2H")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(status, base + o_st, (size_t)n * 4, cudaMemcpyDeviceToHost, st), "D2H")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(out, base + o_out, out_end, cudaMemcpyDeviceToHost, st), "D2H")) return HGPU_ERR_CUDA;
+    if (hgpu_d2h(out_len, L.at(s_olen), (size_t)n * 4, st) || hgpu_d2h(status, L.at(s_st), (size_t)n * 4, st) ||
+        hgpu_d2h(out, L.at(s_out), out_end, st)) return HGPU_ERR_CUDA;
     if (hgpu_check(cudaStreamSynchronize(st), "sync")) return HGPU_ERR_CUDA;
     return HGPU_OK;
 }
 
-// no C++ exception may cross the C ABI (host buffers are sized from untrusted input: std::bad_alloc)
 extern "C" int hgpu_fqz_encode_batch_host(hgpu_ctx *ctx, const uint8_t *in, const uint64_t *in_off, const uint32_t *in_len,
         const uint32_t *rec_len, const uint64_t *rec_off, const uint32_t *nrec, uint32_t n, int strat,
         uint8_t *out, const uint64_t *out_off, const uint32_t *out_cap, uint32_t *out_len, int32_t *status)
 {
-    try {
+    return hgpu_abi_call([&] {
         return hgpu_fqz_encode_batch_host_impl(ctx, in, in_off, in_len, rec_len, rec_off, nrec, n, strat, out, out_off, out_cap, out_len, status);
-    } catch (const std::bad_alloc &) {
-        hgpu_set_error("out of host memory");
-        return HGPU_ERR_NOMEM;
-    } catch (...) {
-        hgpu_set_error("internal error");
-        return HGPU_ERR_CUDA;
-    }
+    });
 }

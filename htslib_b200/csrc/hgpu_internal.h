@@ -3,7 +3,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stddef.h>
+#include <new>
+#include <type_traits>
 #include "../../include/htsgpu.h"
+#include "stage_layout.h"
 
 #define HGPU_WARP 32
 
@@ -36,8 +39,89 @@ int  hgpu_ensure_pinned(hgpu_ctx *ctx, size_t bytes);
 void hgpu_shim_lock();
 void hgpu_shim_unlock();
 hgpu_ctx *hgpu_shim_ctx();
+struct ShimLock { ShimLock() { hgpu_shim_lock(); } ~ShimLock() { hgpu_shim_unlock(); } };
 // a zeroed (stream-ordered) work counter; slots rotate so launches in flight on different streams never share one
 uint32_t *hgpu_take_counter(hgpu_ctx *ctx, cudaStream_t st);
+
+// Grows ctx->d_stage to L.total and binds L to it.  *moved (may be NULL): the buffer was reallocated, so whatever was
+// uploaded into it before this call is gone (a new allocation may land on the old address: capacities are compared).
+inline int hgpu_stage_ensure(hgpu_ctx *ctx, StageLayout &L, bool *moved = nullptr)
+{
+    const size_t cap = ctx->d_stage_cap;
+    const int rc = hgpu_ensure_stage(ctx, L.total);
+    if (moved) *moved = ctx->d_stage_cap != cap;
+    L.base = ctx->d_stage;
+    return rc;
+}
+
+// Checked stream-ordered copies: HGPU_OK, or HGPU_ERR_CUDA with the error text set.  Zero-byte copies are skipped.
+inline int hgpu_h2d(void *dst, const void *src, size_t n, cudaStream_t s)
+{
+    return n ? hgpu_check(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, s), "H2D") : HGPU_OK;
+}
+inline int hgpu_d2h(void *dst, const void *src, size_t n, cudaStream_t s)
+{
+    return n ? hgpu_check(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, s), "D2H") : HGPU_OK;
+}
+inline int hgpu_memset(void *dst, int v, size_t n, cudaStream_t s)
+{
+    return n ? hgpu_check(cudaMemsetAsync(dst, v, n, s), "memset") : HGPU_OK;
+}
+
+// max(off[i] + len[i]): how far into a caller's buffer a batch of slots reaches
+inline uint64_t hgpu_slots_end(const uint64_t *off, const uint32_t *len, uint32_t n)
+{
+    uint64_t e = 0;
+    for (uint32_t i = 0; i < n; i++) if (off[i] + len[i] > e) e = off[i] + len[i];
+    return e;
+}
+
+// No C++ exception may cross the C ABI (host buffers are sized from untrusted input: std::bad_alloc).  Every extern "C"
+// entry point that allocates runs its body through this; the codes are what that entry point documents for each case.
+template <class F> using hgpu_result_t = std::invoke_result_t<F &>;
+template <class F>
+hgpu_result_t<F> hgpu_abi_call(F &&f, hgpu_result_t<F> on_nomem = HGPU_ERR_NOMEM, hgpu_result_t<F> on_other = HGPU_ERR_CUDA)
+{
+    try {
+        return f();
+    } catch (const std::bad_alloc &) {
+        hgpu_set_error("out of host memory");
+        return on_nomem;
+    } catch (...) {
+        hgpu_set_error("internal error");
+        return on_other;
+    }
+}
+
+// The two readers of htscodecs' big-endian 7-bit varints (varint.h).  They differ on truncated and over-long input,
+// and each caller keeps the one whose result it has always had.
+// var_get_u32 as the reference has it (varint.h:267-299): six or more bytes left -> up to six read without a bound check.
+inline int hgpu_var_get_u32(const uint8_t *p, const uint8_t *end, uint32_t *v)
+{
+    const uint8_t *s = p;
+    uint32_t acc = 0;
+    uint8_t c;
+    if (end - p >= 6) {
+        int n = 5;
+        do { c = *p++; acc = (acc << 7) | (c & 0x7f); } while ((c & 0x80) && n-- > 0);
+    } else {
+        if (p >= end) { *v = 0; return 0; }
+        if (*p < 128) { *v = *p; return 1; }
+        do { c = *p++; acc = (acc << 7) | (c & 0x7f); } while ((c & 0x80) && p < end);
+    }
+    *v = acc;
+    return (int)(p - s);
+}
+// The groups var_put_u32 writes (varint.h:206), every byte checked against end, at most six read.
+inline int hgpu_var_get_u32_bounded(const uint8_t *p, const uint8_t *end, uint32_t *v)
+{
+    const uint8_t *s = p;
+    uint32_t acc = 0, c;
+    int n = 0;
+    do { if (p >= end) { *v = acc; return (int)(p - s); } c = *p++; acc = (acc << 7) | (c & 0x7f); } while ((c & 0x80) && ++n < 6);
+    *v = acc;
+    return (int)(p - s);
+}
 
 // kernel launchers (one per .cu)
 int hgpu_launch_rans_nx16(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off,

@@ -20,10 +20,6 @@
 #include <vector>
 #include <string.h>
 
-extern "C" int hgpu_rans_nx16_encode_batch_dev(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off,
-        const uint32_t *d_in_len, const uint32_t *d_order, uint32_t n, uint8_t *d_out, const uint64_t *d_out_off,
-        const uint32_t *d_out_cap, uint32_t *d_out_len, int32_t *d_status, void *stream);
-
 namespace {
 
 constexpr uint32_t NSTREAM = TOK_MAX * 16;
@@ -171,34 +167,27 @@ static int hgpu_tok3_encode_batch_host_impl(hgpu_ctx *ctx, const uint8_t *in, co
     if (n == 0) return HGPU_OK;
     if (hgpu_check(cudaSetDevice(ctx->device), "cudaSetDevice")) return HGPU_ERR_CUDA;
     cudaStream_t s = ctx->stream;
-    auto up = [](uint64_t x) { return (x + 255) & ~(uint64_t)255; };
 
     // ---- pass 0: sizes of every (position, type) stream
-    uint64_t in_end = 0;
-    for (uint32_t b = 0; b < n; b++) if (in_off[b] + in_len[b] > in_end) in_end = in_off[b] + in_len[b];
-    const uint64_t o_in = 0, o_ioff = o_in + up(in_end + 8), o_ilen = o_ioff + up((uint64_t)n * 8), o_cnt = o_ilen + up((uint64_t)n * 4),
-                   o_soff = o_cnt + up((uint64_t)n * NSTREAM * 4), o_meta = o_soff + up((uint64_t)n * NSTREAM * 4),
-                   o_aoff = o_meta + up((uint64_t)n * sizeof(EncMeta)), fixed_end = o_aoff + up((uint64_t)n * 8);
+    const uint64_t in_end = hgpu_slots_end(in_off, in_len, n);
+    StageLayout L;
+    const auto s_in = L.seg(in_end + 8), s_ioff = L.seg((size_t)n * 8), s_ilen = L.seg((size_t)n * 4), s_cnt = L.seg((size_t)n * NSTREAM * 4),
+               s_soff = L.seg((size_t)n * NSTREAM * 4), s_meta = L.seg((size_t)n * sizeof(EncMeta)), s_aoff = L.seg((size_t)n * 8);
+    const size_t fixed_end = L.total;
     // the stream arena (each stream 16-byte aligned) is sized from the counts of pass 0, which does not touch it
     std::vector<uint64_t> aoff(n, 0);
-    uint64_t arena = 0;
-    int rc = hgpu_ensure_stage(ctx, fixed_end + 4096);
+    StageLayout arena;                             // one 256-byte-aligned region per block
+    int rc = hgpu_stage_ensure(ctx, L);
     if (rc) return rc;
-    uint8_t *base = ctx->d_stage;
-    if (hgpu_check(cudaMemcpyAsync(base + o_in, in, in_end, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(base + o_ioff, in_off, (size_t)n * 8, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(base + o_ilen, in_len, (size_t)n * 4, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemsetAsync(base + o_cnt, 0, (size_t)n * NSTREAM * 4, s), "memset")) return HGPU_ERR_CUDA;
-    uint32_t *d_cnt = (uint32_t *)(base + o_cnt), *d_soff = (uint32_t *)(base + o_soff);
-    uint8_t *d_arena = base + fixed_end;
-    tok3_tokenise_kernel<0><<<(n + 31) / 32, 32, 0, s>>>(base + o_in, (const uint64_t *)(base + o_ioff), (const uint32_t *)(base + o_ilen), n,
-                                                         d_cnt, d_soff, d_arena, (const uint64_t *)(base + o_aoff), (EncMeta *)(base + o_meta));
+    if (hgpu_h2d(L.at(s_in), in, in_end, s) || hgpu_h2d(L.at(s_ioff), in_off, (size_t)n * 8, s) || hgpu_h2d(L.at(s_ilen), in_len, (size_t)n * 4, s) ||
+        hgpu_memset(L.at(s_cnt), 0, (size_t)n * NSTREAM * 4, s)) return HGPU_ERR_CUDA;
+    tok3_tokenise_kernel<0><<<(n + 31) / 32, 32, 0, s>>>(L.at(s_in), L.at<uint64_t>(s_ioff), L.at<uint32_t>(s_ilen), n, L.at<uint32_t>(s_cnt),
+                                                         L.at<uint32_t>(s_soff), L.base + fixed_end, L.at<uint64_t>(s_aoff), L.at<EncMeta>(s_meta));
     if (hgpu_check(cudaGetLastError(), "tok3_tokenise_kernel<0>")) return HGPU_ERR_CUDA;
     hgpu_count_launch();
     std::vector<uint32_t> cnt((size_t)n * NSTREAM), soff((size_t)n * NSTREAM, 0);
     std::vector<EncMeta> meta(n);
-    if (hgpu_check(cudaMemcpyAsync(cnt.data(), d_cnt, cnt.size() * 4, cudaMemcpyDeviceToHost, s), "D2H")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(meta.data(), base + o_meta, (size_t)n * sizeof(EncMeta), cudaMemcpyDeviceToHost, s), "D2H")) return HGPU_ERR_CUDA;
+    if (hgpu_d2h(cnt.data(), L.at(s_cnt), cnt.size() * 4, s) || hgpu_d2h(meta.data(), L.at(s_meta), (size_t)n * sizeof(EncMeta), s)) return HGPU_ERR_CUDA;
     if (hgpu_check(cudaStreamSynchronize(s), "sync")) return HGPU_ERR_CUDA;
 
     // ---- layout + the entropy-coder job list: each stream once with order 0, streams of >= 64 bytes also with order 1
@@ -208,7 +197,7 @@ static int hgpu_tok3_encode_batch_host_impl(hgpu_ctx *ctx, const uint8_t *in, co
     std::vector<uint32_t> jil, jord, jcap;
     uint64_t comp_bytes = 0;
     for (uint32_t b = 0; b < n; b++) {
-        aoff[b] = arena;
+        aoff[b] = arena.total;
         if (meta[b].status) continue;
         uint32_t o = 0;
         for (uint32_t id = 0; id < meta[b].max_tok * 16 && id < NSTREAM; id++) {
@@ -227,7 +216,7 @@ static int hgpu_tok3_encode_batch_host_impl(hgpu_ctx *ctx, const uint8_t *in, co
                 for (int q = 0; q < 2; q++) { const int m = k_l3[ty][q]; if (m > 1 && (!(m & 8) || c % 4 == 0)) ords[no++] = (uint32_t)m; }
             StreamRef r{b, id, (uint32_t)jio.size(), no};
             for (uint32_t k = 0; k < r.njobs; k++) {
-                jio.push_back(fixed_end + aoff[b] + o);                          // relative to base + o_in (= base), the encoder's d_in
+                jio.push_back(fixed_end + aoff[b] + o);                          // relative to the input's region (at 0), the encoder's d_in
                 jil.push_back(c); jord.push_back(ords[k]);
                 const uint32_t cap = c + 256;                                    // every level of the coder falls back to CAT, so c + framing is enough
                 joo.push_back(comp_bytes); jcap.push_back(cap);
@@ -236,47 +225,38 @@ static int hgpu_tok3_encode_batch_host_impl(hgpu_ctx *ctx, const uint8_t *in, co
             streams.push_back(r);
             o += (c + 15) & ~15u;
         }
-        arena += up((uint64_t)o + 16);
+        arena.seg((size_t)o + 16);
     }
     const uint32_t nj = (uint32_t)jio.size();
-    // second staging region behind the arena: job arrays and the compressed streams
-    const uint64_t o_jio = fixed_end + up(arena + 64), o_joo = o_jio + up((uint64_t)nj * 8), o_jil = o_joo + up((uint64_t)nj * 8),
-                   o_jord = o_jil + up((uint64_t)nj * 4), o_jcap = o_jord + up((uint64_t)nj * 4), o_jlen = o_jcap + up((uint64_t)nj * 4),
-                   o_jst = o_jlen + up((uint64_t)nj * 4), o_comp = o_jst + up((uint64_t)nj * 4), total = o_comp + up(comp_bytes + 64);
-    // growing the staging buffer would move it: the arena must be rebuilt by pass 1 anyway, but the input has to be re-uploaded
-    const size_t cap_before = ctx->d_stage_cap;      // (a re-allocation may land on the same address: compare capacities, not pointers)
-    rc = hgpu_ensure_stage(ctx, total + 4096);
+    // second part of the staging layout, behind the arena: job arrays and the compressed streams
+    L.seg(arena.total + 64);
+    const auto s_jio = L.seg((size_t)nj * 8), s_joo = L.seg((size_t)nj * 8), s_jil = L.seg((size_t)nj * 4), s_jord = L.seg((size_t)nj * 4),
+               s_jcap = L.seg((size_t)nj * 4), s_jlen = L.seg((size_t)nj * 4), s_jst = L.seg((size_t)nj * 4), s_comp = L.seg(comp_bytes + 64);
+    // growing the staging buffer moves it: the arena is rebuilt by pass 1 anyway, but the input has to be uploaded again
+    bool moved = false;
+    rc = hgpu_stage_ensure(ctx, L, &moved);
     if (rc) return rc;
-    base = ctx->d_stage;
-    if (ctx->d_stage_cap != cap_before) {
-        if (hgpu_check(cudaMemcpyAsync(base + o_in, in, in_end, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(base + o_ioff, in_off, (size_t)n * 8, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(base + o_ilen, in_len, (size_t)n * 4, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-    }
-    if (hgpu_check(cudaMemcpyAsync(base + o_aoff, aoff.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-    d_cnt = (uint32_t *)(base + o_cnt); d_soff = (uint32_t *)(base + o_soff); d_arena = base + fixed_end;
-    if (hgpu_check(cudaMemsetAsync(d_cnt, 0, (size_t)n * NSTREAM * 4, s), "memset")) return HGPU_ERR_CUDA;
-    if (hgpu_check(cudaMemcpyAsync(d_soff, soff.data(), soff.size() * 4, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-    tok3_tokenise_kernel<1><<<(n + 31) / 32, 32, 0, s>>>(base + o_in, (const uint64_t *)(base + o_ioff), (const uint32_t *)(base + o_ilen), n,
-                                                         d_cnt, d_soff, d_arena, (const uint64_t *)(base + o_aoff), (EncMeta *)(base + o_meta));
+    if (moved && (hgpu_h2d(L.at(s_in), in, in_end, s) || hgpu_h2d(L.at(s_ioff), in_off, (size_t)n * 8, s) ||
+                  hgpu_h2d(L.at(s_ilen), in_len, (size_t)n * 4, s))) return HGPU_ERR_CUDA;
+    if (hgpu_h2d(L.at(s_aoff), aoff.data(), (size_t)n * 8, s) || hgpu_memset(L.at(s_cnt), 0, (size_t)n * NSTREAM * 4, s) ||
+        hgpu_h2d(L.at(s_soff), soff.data(), soff.size() * 4, s)) return HGPU_ERR_CUDA;
+    tok3_tokenise_kernel<1><<<(n + 31) / 32, 32, 0, s>>>(L.at(s_in), L.at<uint64_t>(s_ioff), L.at<uint32_t>(s_ilen), n, L.at<uint32_t>(s_cnt),
+                                                         L.at<uint32_t>(s_soff), L.base + fixed_end, L.at<uint64_t>(s_aoff), L.at<EncMeta>(s_meta));
     if (hgpu_check(cudaGetLastError(), "tok3_tokenise_kernel<1>")) return HGPU_ERR_CUDA;
     hgpu_count_launch();
     std::vector<uint32_t> jlen(nj);
     std::vector<int32_t> jst(nj);
     std::vector<uint8_t> comp(comp_bytes + 64);
     if (nj) {
-        if (hgpu_check(cudaMemcpyAsync(base + o_jio, jio.data(), (size_t)nj * 8, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(base + o_joo, joo.data(), (size_t)nj * 8, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(base + o_jil, jil.data(), (size_t)nj * 4, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(base + o_jord, jord.data(), (size_t)nj * 4, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(base + o_jcap, jcap.data(), (size_t)nj * 4, cudaMemcpyHostToDevice, s), "H2D")) return HGPU_ERR_CUDA;
-        rc = hgpu_rans_nx16_encode_batch_dev(ctx, base + o_in, (const uint64_t *)(base + o_jio), (const uint32_t *)(base + o_jil),
-                                             (const uint32_t *)(base + o_jord), nj, base + o_comp, (const uint64_t *)(base + o_joo),
-                                             (const uint32_t *)(base + o_jcap), (uint32_t *)(base + o_jlen), (int32_t *)(base + o_jst), s);
+        if (hgpu_h2d(L.at(s_jio), jio.data(), (size_t)nj * 8, s) || hgpu_h2d(L.at(s_joo), joo.data(), (size_t)nj * 8, s) ||
+            hgpu_h2d(L.at(s_jil), jil.data(), (size_t)nj * 4, s) || hgpu_h2d(L.at(s_jord), jord.data(), (size_t)nj * 4, s) ||
+            hgpu_h2d(L.at(s_jcap), jcap.data(), (size_t)nj * 4, s)) return HGPU_ERR_CUDA;
+        rc = hgpu_rans_nx16_encode_batch_dev(ctx, L.at(s_in), L.at<uint64_t>(s_jio), L.at<uint32_t>(s_jil), L.at<uint32_t>(s_jord), nj,
+                                             L.at(s_comp), L.at<uint64_t>(s_joo), L.at<uint32_t>(s_jcap), L.at<uint32_t>(s_jlen),
+                                             L.at<int32_t>(s_jst), s);
         if (rc) return rc;
-        if (hgpu_check(cudaMemcpyAsync(jlen.data(), base + o_jlen, (size_t)nj * 4, cudaMemcpyDeviceToHost, s), "D2H")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(jst.data(), base + o_jst, (size_t)nj * 4, cudaMemcpyDeviceToHost, s), "D2H")) return HGPU_ERR_CUDA;
-        if (hgpu_check(cudaMemcpyAsync(comp.data(), base + o_comp, comp_bytes, cudaMemcpyDeviceToHost, s), "D2H")) return HGPU_ERR_CUDA;
+        if (hgpu_d2h(jlen.data(), L.at(s_jlen), (size_t)nj * 4, s) || hgpu_d2h(jst.data(), L.at(s_jst), (size_t)nj * 4, s) ||
+            hgpu_d2h(comp.data(), L.at(s_comp), comp_bytes, s)) return HGPU_ERR_CUDA;
     }
     if (hgpu_check(cudaStreamSynchronize(s), "sync")) return HGPU_ERR_CUDA;
 
@@ -313,17 +293,8 @@ static int hgpu_tok3_encode_batch_host_impl(hgpu_ctx *ctx, const uint8_t *in, co
     return HGPU_OK;
 }
 
-// no C++ exception may cross the C ABI (host buffers are sized from untrusted input: std::bad_alloc)
 extern "C" int hgpu_tok3_encode_batch_host(hgpu_ctx *ctx, const uint8_t *in, const uint64_t *in_off, const uint32_t *in_len,
         uint32_t n, uint8_t *out, const uint64_t *out_off, const uint32_t *out_cap, uint32_t *out_len, int32_t *status)
 {
-    try {
-        return hgpu_tok3_encode_batch_host_impl(ctx, in, in_off, in_len, n, out, out_off, out_cap, out_len, status);
-    } catch (const std::bad_alloc &) {
-        hgpu_set_error("out of host memory");
-        return HGPU_ERR_NOMEM;
-    } catch (...) {
-        hgpu_set_error("internal error");
-        return HGPU_ERR_CUDA;
-    }
+    return hgpu_abi_call([&] { return hgpu_tok3_encode_batch_host_impl(ctx, in, in_off, in_len, n, out, out_off, out_cap, out_len, status); });
 }

@@ -14,8 +14,6 @@
 
 namespace {
 
-struct ShimLock { ShimLock() { hgpu_shim_lock(); } ~ShimLock() { hgpu_shim_unlock(); } };
-
 // ---- unpack: out[i] = map[field i of data]; fully parallel
 __global__ void xf_unpack_kernel(const uint8_t *d, uint64_t len, uint8_t *out, uint64_t olen, int per_byte, const uint8_t *map)
 {
@@ -123,19 +121,18 @@ __global__ void xf_rle_decode_kernel(const uint8_t *lit, uint64_t nlit, const ui
     if (lane == 0) res[0] = bad ? ~0ull : o;
 }
 
-// device staging for one call: [a | b | c | small] regions in ctx->d_stage
+// binds one call's layout to the staging buffer of the process-wide shim context
 struct Stage {
-    hgpu_ctx *ctx; uint8_t *base; cudaStream_t s;
+    hgpu_ctx *ctx; cudaStream_t s;
     bool ok;
-    Stage(size_t bytes) : ctx(hgpu_shim_ctx()), base(nullptr), s(nullptr), ok(false)
+    Stage(StageLayout &L) : ctx(hgpu_shim_ctx()), s(nullptr), ok(false)
     {
         if (!ctx) return;
         if (cudaSetDevice(ctx->device) != cudaSuccess) return;
-        if (hgpu_ensure_stage(ctx, bytes + 4096)) return;
-        base = ctx->d_stage; s = ctx->stream; ok = true;
+        if (hgpu_stage_ensure(ctx, L)) return;
+        s = ctx->stream; ok = true;
     }
 };
-inline size_t up(size_t x) { return (x + 255) & ~(size_t)255; }
 
 }  // namespace
 
@@ -170,14 +167,15 @@ uint8_t *hts_unpack(uint8_t *data, int64_t len, uint8_t *out, uint64_t out_len, 
     if (out_len == 0) return out;
     ShimLock lock;
     try {
-        Stage st(up((size_t)len) + up(out_len) + 256);
+        StageLayout L;
+        const auto s_in = L.seg((size_t)len), s_out = L.seg(out_len), s_map = L.seg(16);
+        Stage st(L);
         if (!st.ok) return nullptr;
-        uint8_t *d_in = st.base, *d_out = d_in + up((size_t)len), *d_map = d_out + up(out_len);
-        if (len && hgpu_check(cudaMemcpyAsync(d_in, data, (size_t)len, cudaMemcpyHostToDevice, st.s), "H2D")) return nullptr;
-        if (hgpu_check(cudaMemcpyAsync(d_map, map, 16, cudaMemcpyHostToDevice, st.s), "H2D")) return nullptr;
+        uint8_t *d_in = L.at(s_in), *d_out = L.at(s_out), *d_map = L.at(s_map);
+        if (hgpu_h2d(d_in, data, (size_t)len, st.s) || hgpu_h2d(d_map, map, 16, st.s)) return nullptr;
         xf_unpack_kernel<<<(unsigned)((out_len + 255) / 256 < 4096 ? (out_len + 255) / 256 : 4096), 256, 0, st.s>>>(d_in, (uint64_t)len, d_out, out_len, nsym, d_map);
         hgpu_count_launch();
-        if (hgpu_check(cudaGetLastError(), "xf_unpack") || hgpu_check(cudaMemcpyAsync(out, d_out, out_len, cudaMemcpyDeviceToHost, st.s), "D2H") ||
+        if (hgpu_check(cudaGetLastError(), "xf_unpack") || hgpu_d2h(out, d_out, out_len, st.s) ||
             hgpu_check(cudaStreamSynchronize(st.s), "sync")) return nullptr;
         return out;
     } catch (...) { return nullptr; }
@@ -188,15 +186,16 @@ uint8_t *hts_pack(uint8_t *data, int64_t len, uint8_t *out_meta, int *out_meta_l
     if (len < 0 || (len && !data) || !out_meta || !out_meta_len || !out_len) return nullptr;
     ShimLock lock;
     try {
-        Stage st(up((size_t)len) + up((size_t)len + 1) + 2048);
-        if (!st.ok) return nullptr;
-        uint8_t *d_in = st.base, *d_out = d_in + up((size_t)len), *d_code = d_out + up((size_t)len + 1);
-        uint32_t *d_present = (uint32_t *)(d_code + 256);
         uint32_t present[256];
-        if (len && hgpu_check(cudaMemcpyAsync(d_in, data, (size_t)len, cudaMemcpyHostToDevice, st.s), "H2D")) return nullptr;
-        if (hgpu_check(cudaMemsetAsync(d_present, 0, sizeof(present), st.s), "memset")) return nullptr;
+        StageLayout L;
+        const auto s_in = L.seg((size_t)len), s_out = L.seg((size_t)len + 1), s_code = L.seg(256), s_present = L.seg(sizeof(present));
+        Stage st(L);
+        if (!st.ok) return nullptr;
+        uint8_t *d_in = L.at(s_in), *d_out = L.at(s_out), *d_code = L.at(s_code);
+        uint32_t *d_present = L.at<uint32_t>(s_present);
+        if (hgpu_h2d(d_in, data, (size_t)len, st.s) || hgpu_memset(d_present, 0, sizeof(present), st.s)) return nullptr;
         if (len) { xf_present_kernel<<<(unsigned)(((uint64_t)len + 255) / 256 < 4096 ? ((uint64_t)len + 255) / 256 : 4096), 256, 0, st.s>>>(d_in, (uint64_t)len, d_present); hgpu_count_launch(); }
-        if (hgpu_check(cudaMemcpyAsync(present, d_present, sizeof(present), cudaMemcpyDeviceToHost, st.s), "D2H") || hgpu_check(cudaStreamSynchronize(st.s), "sync")) return nullptr;
+        if (hgpu_d2h(present, d_present, sizeof(present), st.s) || hgpu_check(cudaStreamSynchronize(st.s), "sync")) return nullptr;
         uint8_t code[256];
         int n = 0;
         for (int i = 0; i < 256; i++) if (present[i]) { code[i] = (uint8_t)n++; out_meta[n] = (uint8_t)i; } else code[i] = 0;
@@ -208,10 +207,10 @@ uint8_t *hts_pack(uint8_t *data, int64_t len, uint8_t *out_meta, int *out_meta_l
         *out_meta_len = n + 1;
         const uint64_t olen = per ? ((uint64_t)len + per - 1) / per : 0;
         if (olen) {
-            if (hgpu_check(cudaMemcpyAsync(d_code, code, 256, cudaMemcpyHostToDevice, st.s), "H2D")) { free(out); return nullptr; }
+            if (hgpu_h2d(d_code, code, 256, st.s)) { free(out); return nullptr; }
             xf_pack_kernel<<<(unsigned)((olen + 255) / 256 < 4096 ? (olen + 255) / 256 : 4096), 256, 0, st.s>>>(d_in, (uint64_t)len, d_out, olen, per, d_code);
             hgpu_count_launch();
-            if (hgpu_check(cudaGetLastError(), "xf_pack") || hgpu_check(cudaMemcpyAsync(out, d_out, olen, cudaMemcpyDeviceToHost, st.s), "D2H") ||
+            if (hgpu_check(cudaGetLastError(), "xf_pack") || hgpu_d2h(out, d_out, olen, st.s) ||
                 hgpu_check(cudaStreamSynchronize(st.s), "sync")) { free(out); return nullptr; }
         }
         *out_len = olen;
@@ -226,35 +225,37 @@ uint8_t *hts_rle_encode(uint8_t *data, uint64_t data_len, uint8_t *run, uint64_t
     ShimLock lock;
     try {
         // worst cases: literals data_len bytes, run lengths one byte per literal
-        Stage st(up(data_len) * 3 + 4096);
+        StageLayout L;
+        const auto s_in = L.seg(data_len), s_lit = L.seg(data_len), s_run = L.seg(data_len), s_set = L.seg(256), s_saved = L.seg(256 * sizeof(int)),
+                   s_lens = L.seg(16);
+        Stage st(L);
         if (!st.ok) return nullptr;
-        uint8_t *d_in = st.base, *d_lit = d_in + up(data_len), *d_run = d_lit + up(data_len), *d_set = d_run + up(data_len);
-        int *d_saved = (int *)(d_set + 256);
-        uint64_t *d_lens = (uint64_t *)(d_set + 256 + 1024);
-        if (data_len && hgpu_check(cudaMemcpyAsync(d_in, data, data_len, cudaMemcpyHostToDevice, st.s), "H2D")) return nullptr;
+        uint8_t *d_in = L.at(s_in), *d_lit = L.at(s_lit), *d_run = L.at(s_run), *d_set = L.at(s_set);
+        int *d_saved = L.at<int>(s_saved);
+        uint64_t *d_lens = L.at<uint64_t>(s_lens);
+        if (hgpu_h2d(d_in, data, data_len, st.s)) return nullptr;
         uint8_t inset[256] = {0};
         if (*rle_nsyms) { for (int i = 0; i < *rle_nsyms; i++) inset[rle_syms[i]] = 1; }
         else {
             int saved[256];
-            if (hgpu_check(cudaMemsetAsync(d_saved, 0, sizeof(saved), st.s), "memset")) return nullptr;
+            if (hgpu_memset(d_saved, 0, sizeof(saved), st.s)) return nullptr;
             if (data_len) { xf_rle_survey_kernel<<<(unsigned)((data_len + 255) / 256 < 1024 ? (data_len + 255) / 256 : 1024), 256, 0, st.s>>>(d_in, data_len, d_saved); hgpu_count_launch(); }
-            if (hgpu_check(cudaMemcpyAsync(saved, d_saved, sizeof(saved), cudaMemcpyDeviceToHost, st.s), "D2H") || hgpu_check(cudaStreamSynchronize(st.s), "sync")) return nullptr;
+            if (hgpu_d2h(saved, d_saved, sizeof(saved), st.s) || hgpu_check(cudaStreamSynchronize(st.s), "sync")) return nullptr;
             int n = 0;
             for (int i = 0; i < 256; i++) if (saved[i] > 0) { rle_syms[n++] = (uint8_t)i; inset[i] = 1; }
             *rle_nsyms = n;
         }
         uint64_t lens[2] = {0, 0};
         if (data_len) {
-            if (hgpu_check(cudaMemcpyAsync(d_set, inset, 256, cudaMemcpyHostToDevice, st.s), "H2D")) return nullptr;
+            if (hgpu_h2d(d_set, inset, 256, st.s)) return nullptr;
             xf_rle_encode_kernel<<<1, 32, 0, st.s>>>(d_in, data_len, d_set, d_lit, d_run, d_lens);
             hgpu_count_launch();
-            if (hgpu_check(cudaGetLastError(), "xf_rle_encode") || hgpu_check(cudaMemcpyAsync(lens, d_lens, sizeof(lens), cudaMemcpyDeviceToHost, st.s), "D2H") ||
+            if (hgpu_check(cudaGetLastError(), "xf_rle_encode") || hgpu_d2h(lens, d_lens, sizeof(lens), st.s) ||
                 hgpu_check(cudaStreamSynchronize(st.s), "sync")) return nullptr;
         }
         bool mine = false;
         if (!out) { out = (uint8_t *)malloc(data_len * 2 + 1); if (!out) return nullptr; mine = true; }
-        if ((lens[0] && hgpu_check(cudaMemcpyAsync(out, d_lit, lens[0], cudaMemcpyDeviceToHost, st.s), "D2H")) ||
-            (lens[1] && hgpu_check(cudaMemcpyAsync(run, d_run, lens[1], cudaMemcpyDeviceToHost, st.s), "D2H")) ||
+        if (hgpu_d2h(out, d_lit, lens[0], st.s) || hgpu_d2h(run, d_run, lens[1], st.s) ||
             hgpu_check(cudaStreamSynchronize(st.s), "sync")) { if (mine) free(out); return nullptr; }
         *out_len = lens[0];
         *run_len = lens[1];
@@ -270,22 +271,22 @@ uint8_t *hts_rle_decode(uint8_t *lit, uint64_t lit_len, uint8_t *run, uint64_t r
     ShimLock lock;
     try {
         const uint64_t cap = *out_len;
-        Stage st(up(lit_len) + up(run_len) + up(cap) + 1024);
+        StageLayout L;
+        const auto s_lit = L.seg(lit_len), s_run = L.seg(run_len), s_out = L.seg(cap), s_set = L.seg(256), s_res = L.seg(8);
+        Stage st(L);
         if (!st.ok) return nullptr;
-        uint8_t *d_lit = st.base, *d_run = d_lit + up(lit_len), *d_out = d_run + up(run_len), *d_set = d_out + up(cap);
-        uint64_t *d_res = (uint64_t *)(d_set + 256);
+        uint8_t *d_lit = L.at(s_lit), *d_run = L.at(s_run), *d_out = L.at(s_out), *d_set = L.at(s_set);
+        uint64_t *d_res = L.at<uint64_t>(s_res);
         uint8_t inset[256] = {0};
         for (int i = 0; i < rle_nsyms; i++) inset[rle_syms[i]] = 1;
-        if (hgpu_check(cudaMemcpyAsync(d_lit, lit, lit_len, cudaMemcpyHostToDevice, st.s), "H2D") ||
-            (run_len && hgpu_check(cudaMemcpyAsync(d_run, run, run_len, cudaMemcpyHostToDevice, st.s), "H2D")) ||
-            hgpu_check(cudaMemcpyAsync(d_set, inset, 256, cudaMemcpyHostToDevice, st.s), "H2D")) return nullptr;
+        if (hgpu_h2d(d_lit, lit, lit_len, st.s) || hgpu_h2d(d_run, run, run_len, st.s) || hgpu_h2d(d_set, inset, 256, st.s)) return nullptr;
         xf_rle_decode_kernel<<<1, 32, 0, st.s>>>(d_lit, lit_len, d_run, run_len, d_set, d_out, cap, d_res);
         hgpu_count_launch();
         uint64_t res = 0;
-        if (hgpu_check(cudaGetLastError(), "xf_rle_decode") || hgpu_check(cudaMemcpyAsync(&res, d_res, 8, cudaMemcpyDeviceToHost, st.s), "D2H") ||
+        if (hgpu_check(cudaGetLastError(), "xf_rle_decode") || hgpu_d2h(&res, d_res, 8, st.s) ||
             hgpu_check(cudaStreamSynchronize(st.s), "sync")) return nullptr;
         if (res == ~0ull || res > cap) return nullptr;
-        if (res && (hgpu_check(cudaMemcpyAsync(out, d_out, res, cudaMemcpyDeviceToHost, st.s), "D2H") || hgpu_check(cudaStreamSynchronize(st.s), "sync"))) return nullptr;
+        if (res && (hgpu_d2h(out, d_out, res, st.s) || hgpu_check(cudaStreamSynchronize(st.s), "sync"))) return nullptr;
         *out_len = res;
         return out;
     } catch (...) { return nullptr; }

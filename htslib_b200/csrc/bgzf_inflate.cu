@@ -1131,18 +1131,27 @@ int ensure_crc_tables(hgpu_ctx *ctx, cudaStream_t st)
 // BGZF block COMPRESS — stands where bgzf_compress / deflate_block / bgzf_encode_func stand
 // (bgzf.c:624-683, :709, :1330): one warp per <= 0xff00-byte payload, output = a complete BGZF
 // block (18-byte header, raw DEFLATE, CRC32, ISIZE).  Compressed bytes need not match zlib's
-// (SURVEY.md §8c); what is pinned is that zlib / the reference reader inflate them back to the
-// input and that the size stays within a stated ratio (tests/test_gpu_bgzf_compress.py).
+// (SURVEY.md §8c).  tests/test_gpu_bgzf_compress.py pins that every decoder inflates them back and
+// the size ratio to zlib; tests/test_gpu_bgzf_deflate.py pins every block's code construction byte
+// for byte against a restatement of pass 2, and the parse and code lengths against plain references.
+// A negative level is level 6 (the host entry point maps it).
 //
-// level 0  : stored block, exactly what htslib writes at level 0 (bgzf.c:573-580).
-// level >=1: lane-parallel LZ77 + fixed-Huffman codes (BTYPE=1).  Every lane hashes the 4 bytes at
-//            its own position (12-bit hash, 16-bit positions in shared memory), verifies and
-//            extends its candidate (plus the distance-1 candidate, which catches the runs that
-//            dominate quality strings), a greedy in-order selection keeps non-overlapping
-//            matches (ballot + ffs skip over literal stretches), tokens go to a per-warp list;
-//            a second pass turns 32 tokens at a time into <= 31-bit codes, prefix-sums their
-//            bit lengths and ORs them into the output words.  Falls back to a stored block when
-//            that would be smaller (zlib arm does the same, bgzf.c:653-667).
+// level 0 or n < 16: stored block, exactly what htslib writes at level 0 (bgzf.c:573-580).
+// level >= 1, pass 1 (LZ77): 32 positions per step, one per lane.  Each lane with 4 bytes left
+//            hashes them (12-bit hash, 16-bit positions in shared memory; every lane reads before
+//            any lane of the step stores), verifies and extends the candidate (>= 4 bytes), and
+//            extends the distance-1 candidate (>= 3 bytes, runs), keeping the longer.  Matches stop
+//            at n and at 258 bytes.  A greedy in-order walk over the step keeps non-overlapping
+//            matches (ballot + ffs over literal stretches); at level >= 4 a match gives way to a
+//            match at the next byte that is longer by 2 or more (one step of lazy evaluation).
+// pass 2 (codes): token histogram with EOB; lit/len, distance and code-length code lengths by
+//            Huffman on sorted leaves, folded to 15 / 15 / 7 bits (build_lengths); the code-length
+//            sequence run-length coded with 16 / 17 / 18.  The exact bit counts of the fixed and
+//            the dynamic block pick the smaller (fixed on a tie); each lane turns a token into a
+//            code of up to 48 bits and ORs it into the slot at its prefix-summed bit offset.
+//            A stored block replaces the result when the token bits would pass the slot's end or
+//            the result is not smaller than a stored block (the zlib arm does the same,
+//            bgzf.c:653-667).
 // =============================================================================================
 constexpr uint32_t DEFL_HASH_BITS = 12;
 constexpr uint32_t DEFL_MAX_IN = 0xff00 + 256;      // htslib never exceeds 0xff00; allow the full 64 KiB - 280
@@ -1665,6 +1674,7 @@ extern "C" int hgpu_bgzf_compress_batch_dev(hgpu_ctx *ctx, const uint8_t *d_in, 
 {
     if (!ctx) { hgpu_set_error("null context"); return HGPU_ERR_ARG; }
     if (n == 0) return HGPU_OK;
+    if (level < 0) level = 6;                           // Z_DEFAULT_COMPRESSION, as zlib's deflateInit2 reads it
     cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
     int rc = ensure_crc_tables(ctx, st);
     if (rc) return rc;

@@ -631,7 +631,7 @@ extern "C" int bgzf_compress(void *dst, size_t *dlen, const void *src, size_t sl
     int32_t st = 0;
     cudaStream_t s = ctx->stream;
     if (hgpu_h2d(d_in, src, slen, s) || hgpu_h2d(d_off, offs, 16, s) || hgpu_h2d(d_len, &len32, 4, s)) return -1;
-    if (hgpu_bgzf_compress_batch_dev(ctx, d_in, d_off, d_len, 1, level < 0 ? 6 : level, d_out, d_off + 1, d_ol, d_st, s)) return -1;
+    if (hgpu_bgzf_compress_batch_dev(ctx, d_in, d_off, d_len, 1, level, d_out, d_off + 1, d_ol, d_st, s)) return -1;
     if (hgpu_d2h(&got, d_ol, 4, s) || hgpu_d2h(&st, d_st, 4, s)) return -1;
     if (cudaStreamSynchronize(s) != cudaSuccess) return -1;
     if (st != HGPU_OK || got == 0 || got > *dlen) return -1;

@@ -85,9 +85,12 @@ int hgpu_bgzf_inflate_jobs_host(hgpu_ctx *ctx, uint32_t n, const uint8_t *const 
  * BGZF_BLOCK_SIZE 0xff00), one warp per payload.  Every out slot is 65536 bytes, 4-byte aligned;
  * out_len[i] receives the BGZF block length.  level 0 = stored block (bgzf.c:573-580), level >= 1 =
  * LZ77 tokens coded by the smallest of a dynamic-Huffman block (code lengths built per block on the device), a
- * fixed-Huffman block and a stored block.  Output inflates to the input with any RFC 1951 inflater; bytes differ
- * from zlib's (stated ratio in tests/test_gpu_bgzf_compress.py: 1.12x the zlib level-6 size on sorted BAM at level >= 4,
- * where one step of lazy match evaluation is on). */
+ * fixed-Huffman block and a stored block; levels 1-3 parse greedily, levels >= 4 add one step of lazy evaluation.
+ * A negative level means level 6, as Z_DEFAULT_COMPRESSION (-1) does for zlib; htslib's writer passes -1 by default.
+ * A payload over 65280 bytes gets status HGPU_BGZF_ERR_ZLIB and out_len 0; the other jobs are unaffected.
+ * Output inflates to the input with any RFC 1951 inflater; bytes differ from zlib's (stated ratio in
+ * tests/test_gpu_bgzf_compress.py: 1.12x the zlib level-6 size on sorted BAM at level >= 4).  tests/test_gpu_bgzf_deflate.py
+ * checks every block's code construction byte for byte against a restatement (tests/deflate_model.py). */
 int hgpu_bgzf_compress_batch_dev(hgpu_ctx *ctx,
         const uint8_t *d_in, const uint64_t *d_in_off, const uint32_t *d_in_len, uint32_t n, int level,
         uint8_t *d_out, const uint64_t *d_out_off, uint32_t *d_out_len, int32_t *d_status, void *stream);
@@ -559,7 +562,8 @@ char *fqz_compress(int vers, void *slice, char *in, size_t uncomp_size, size_t *
 uint32_t hts_crc32(uint32_t crc, const void *buf, size_t len);
 /* bgzf_compress (htslib/bgzf.h:392, htslib.map:312): one BGZF block from slen <= 65280 bytes;
  * *dlen is capacity in / block length out; slen == 0 writes the 28-byte EOF block (bgzf.c:566);
- * returns 0 or -1.  Host pointers. */
+ * a negative level means level 6 (as hgpu_bgzf_compress_batch_dev); returns 0, or -1 also when *dlen is too
+ * small for the block.  Host pointers. */
 int bgzf_compress(void *dst, size_t *dlen, const void *src, size_t slen, int level);
 
 #ifdef __cplusplus

@@ -13,6 +13,8 @@
  * test/bgzf_boundaries/*.bam, and against the compiled reference's bgzf_read.
  *
  * Decoding is done the slow, obviously-correct way: canonical codes walked one bit at a time.
+ * orc_inflate_trace runs the same decode loop and also reports each block's type, header extent,
+ * code lengths and tokens, so tests can check how an encoder built a block, not only what it holds.
  */
 #include <stdint.h>
 #include <string.h>
@@ -78,18 +80,54 @@ static const uint16_t DST_BASE[30] = {1,2,3,4,5,7,9,13,17,25,33,49,65,97,129,193
 static const uint8_t  DST_XTRA[30] = {0,0,0,0,1,1,2,2,3,3,4,4,5,5,6,6,7,7,8,8,9,9,10,10,11,11,12,12,13,13};
 
 /*
- * Raw inflate of one complete stream.  Returns 0 and *dlen on success; -1 on any error that
- * makes zlib's inflate(Z_FINISH) return something other than Z_STREAM_END (bad data, input
- * exhausted, output longer than dcap).  *consumed = bytes of src used (rounded up).
+ * Optional sink of inflate_stream: what each deflate block said, as decoded.  The caller owns
+ * every array; a block or token past max_blocks / max_toks makes the inflate fail.
+ *   btype[k]      BFINAL | BTYPE << 1
+ *   start_bit[k]  bit position of the block's BFINAL bit
+ *   body_bit[k]   first bit after the block header (after LEN/NLEN for a stored block)
+ *   end_bit[k]    first bit after the block (after the end-of-block code)
+ *   first_tok[k]  index in toks[] of the block's first token (a stored block has none)
+ *   lens[k*339..] lit/len[288], distance[32] and code-length[19] code lengths; zero beyond
+ *                 HLIT / HDIST, the fixed lengths for BTYPE 1, all zero for a stored block
+ *   toks[]        a literal byte, or 1<<31 | length << 16 | distance
  */
-int orc_inflate_raw(const uint8_t *src, uint64_t slen, uint8_t *dst, uint64_t dcap,
-                    uint64_t *dlen, uint64_t *consumed)
+typedef struct {
+    uint32_t max_blocks, max_toks, nblocks, ntoks;
+    uint8_t *btype;
+    uint64_t *start_bit, *body_bit, *end_bit;
+    uint32_t *first_tok;
+    uint8_t *lens;
+    uint32_t *toks;
+} orc_trace;
+
+enum { TRACE_LENS = 288 + 32 + 19 };
+
+static int trace_tok(orc_trace *t, uint32_t tok)
+{
+    if (t->ntoks >= t->max_toks) return -1;
+    t->toks[t->ntoks++] = tok;
+    return 0;
+}
+
+static int inflate_stream(const uint8_t *src, uint64_t slen, uint8_t *dst, uint64_t dcap,
+                          uint64_t *dlen, uint64_t *consumed, orc_trace *t)
 {
     bitsrc b = { src, slen * 8, 0 };
     uint64_t o = 0;
     uint32_t final, type;
+    uint8_t *tl = 0;                                   /* this block's traced lengths */
     do {
+        if (t) {
+            if (t->nblocks >= t->max_blocks) return -1;
+            t->start_bit[t->nblocks] = b.bitpos;
+        }
         if (getbits(&b, 1, &final) || getbits(&b, 2, &type)) return -1;
+        if (t) {
+            tl = t->lens + (uint64_t)t->nblocks * TRACE_LENS;
+            memset(tl, 0, TRACE_LENS);
+            t->btype[t->nblocks] = (uint8_t)(final | type << 1);
+            t->first_tok[t->nblocks] = t->ntoks;
+        }
         if (type == 0) {
             uint32_t len, nlen;
             b.bitpos = (b.bitpos + 7) & ~7ull;
@@ -97,6 +135,7 @@ int orc_inflate_raw(const uint8_t *src, uint64_t slen, uint8_t *dst, uint64_t dc
             if ((len ^ 0xffff) != nlen) return -1;
             if (b.bitpos + 8ull * len > b.nbits) return -1;
             if (o + len > dcap) return -1;
+            if (t) t->body_bit[t->nblocks] = b.bitpos;
             memcpy(dst + o, src + (b.bitpos >> 3), len);
             o += len;
             b.bitpos += 8ull * len;
@@ -126,6 +165,7 @@ int orc_inflate_raw(const uint8_t *src, uint64_t slen, uint8_t *dst, uint64_t dc
                     lens[order[i]] = (uint8_t)v;
                 }
                 if (canon_build(&cl, lens, 19) != 0) return -1;       /* must be complete */
+                if (t) memcpy(tl + 320, lens, 19);
                 n = 0;
                 while (n < (int)(hlit + hdist)) {
                     int sym = canon_decode(&b, &cl);
@@ -154,13 +194,22 @@ int orc_inflate_raw(const uint8_t *src, uint64_t slen, uint8_t *dst, uint64_t dc
                     if (err < 0 || (err > 0 && !(lit.count[1] == 1 && (int)hlit - lit.count[0] == 1))) return -1;
                     err = canon_build(&dist, dl, (int)hdist);
                     if (err < 0 || (err > 0 && !(dist.count[1] == 1 && (int)hdist - dist.count[0] == 1))) return -1;
+                    if (t) { memcpy(tl, lens, hlit); memcpy(tl + 288, dl, hdist); }
                 }
+            }
+            if (t) {
+                if (type == 1) {
+                    for (i = 0; i < 288; i++) tl[i] = i < 144 ? 8 : i < 256 ? 9 : i < 280 ? 7 : 8;
+                    for (i = 0; i < 30; i++) tl[288 + i] = 5;
+                }
+                t->body_bit[t->nblocks] = b.bitpos;
             }
             for (;;) {
                 int sym = canon_decode(&b, &lit);
                 if (sym < 0) return -1;
                 if (sym < 256) {
                     if (o >= dcap) return -1;
+                    if (t && trace_tok(t, (uint32_t)sym)) return -1;
                     dst[o++] = (uint8_t)sym;
                 } else if (sym == 256) break;
                 else {
@@ -176,15 +225,37 @@ int orc_inflate_raw(const uint8_t *src, uint64_t slen, uint8_t *dst, uint64_t dc
                     d = DST_BASE[ds] + xd;
                     if (d > o) return -1;
                     if (o + len > dcap) return -1;
+                    if (t && trace_tok(t, 1u << 31 | len << 16 | d)) return -1;
                     while (len--) { dst[o] = dst[o - d]; o++; }
                 }
             }
         } else
             return -1;
+        if (t) t->end_bit[t->nblocks++] = b.bitpos;
     } while (!final);
     *dlen = o;
     if (consumed) *consumed = (b.bitpos + 7) >> 3;
     return 0;
+}
+
+/*
+ * Raw inflate of one complete stream.  Returns 0 and *dlen on success; -1 on any error that
+ * makes zlib's inflate(Z_FINISH) return something other than Z_STREAM_END (bad data, input
+ * exhausted, output longer than dcap).  *consumed = bytes of src used (rounded up).
+ */
+int orc_inflate_raw(const uint8_t *src, uint64_t slen, uint8_t *dst, uint64_t dcap,
+                    uint64_t *dlen, uint64_t *consumed)
+{
+    return inflate_stream(src, slen, dst, dcap, dlen, consumed, 0);
+}
+
+/* orc_inflate_raw that also reports every block's type, header extent, code lengths and tokens
+ * into *t (nblocks / ntoks are reset here).  Same return value; -1 also when t runs out of room. */
+int orc_inflate_trace(const uint8_t *src, uint64_t slen, uint8_t *dst, uint64_t dcap,
+                      uint64_t *dlen, uint64_t *consumed, orc_trace *t)
+{
+    t->nblocks = t->ntoks = 0;
+    return inflate_stream(src, slen, dst, dcap, dlen, consumed, t);
 }
 
 /* CRC-32 (IEEE 802.3, reflected 0xEDB88320), as zlib's crc32() / hts_crc32 (bgzf.c:620). */

@@ -348,6 +348,43 @@ def orc_inflate_raw(src, cap=65536):
     return bytes(out[: dl.value]), used.value
 
 
+class _OrcTrace(C.Structure):
+    _fields_ = [("max_blocks", C.c_uint32), ("max_toks", C.c_uint32), ("nblocks", C.c_uint32), ("ntoks", C.c_uint32),
+                ("btype", C.POINTER(C.c_uint8)), ("start_bit", C.POINTER(C.c_uint64)), ("body_bit", C.POINTER(C.c_uint64)),
+                ("end_bit", C.POINTER(C.c_uint64)), ("first_tok", C.POINTER(C.c_uint32)), ("lens", C.POINTER(C.c_uint8)),
+                ("toks", C.POINTER(C.c_uint32))]
+
+
+def orc_inflate_trace(src, cap=65536, max_blocks=4096):
+    """Raw inflate with the oracle's per-block trace.  Returns (output, blocks) or (None, None) on an inflate error.
+    Each block is a dict: bfinal, btype, start_bit, body_bit, end_bit, ll (288 lit/len code lengths), dist (32),
+    cl (19, indexed by code-length symbol) and toks, a list of literal bytes (int) and (length, distance) tuples."""
+    import numpy as np
+    o = orc()
+    out = (C.c_uint8 * max(1, cap))()
+    dl = C.c_uint64(0); used = C.c_uint64(0)
+    arrs = dict(btype=(C.c_uint8 * max_blocks)(), start_bit=(C.c_uint64 * max_blocks)(), body_bit=(C.c_uint64 * max_blocks)(),
+                end_bit=(C.c_uint64 * max_blocks)(), first_tok=(C.c_uint32 * max_blocks)(), lens=(C.c_uint8 * (max_blocks * 339))(),
+                toks=(C.c_uint32 * max(1, cap))())
+    t = _OrcTrace(max_blocks, max(1, cap), 0, 0, *(C.cast(arrs[k], C.POINTER(f)) for k, f in
+                  (("btype", C.c_uint8), ("start_bit", C.c_uint64), ("body_bit", C.c_uint64), ("end_bit", C.c_uint64),
+                   ("first_tok", C.c_uint32), ("lens", C.c_uint8), ("toks", C.c_uint32))))
+    rc = o.orc_inflate_trace(buf(src), C.c_uint64(len(src)), out, C.c_uint64(cap), C.byref(dl), C.byref(used), C.byref(t))
+    if rc:
+        return None, None
+    toks = np.frombuffer(arrs["toks"], dtype=np.uint32, count=t.ntoks)
+    lens = np.frombuffer(arrs["lens"], dtype=np.uint8, count=t.nblocks * 339).reshape(-1, 339)
+    blocks = []
+    for k in range(t.nblocks):
+        end = arrs["first_tok"][k + 1] if k + 1 < t.nblocks else t.ntoks
+        tk = toks[arrs["first_tok"][k]:end]
+        blocks.append(dict(bfinal=arrs["btype"][k] & 1, btype=arrs["btype"][k] >> 1, start_bit=arrs["start_bit"][k],
+                           body_bit=arrs["body_bit"][k], end_bit=arrs["end_bit"][k], ll=lens[k, :288].tolist(),
+                           dist=lens[k, 288:320].tolist(), cl=lens[k, 320:].tolist(),
+                           toks=[int(v) if v < 256 else ((int(v) >> 16) & 0x1ff, int(v) & 0xffff) for v in tk]))
+    return bytes(out[: dl.value]), blocks
+
+
 def orc_bgzf_inflate_block(block):
     o = orc()
     out = (C.c_uint8 * 65536)()

@@ -21,7 +21,7 @@ def ctx():
     c.close()
 
 
-@pytest.mark.parametrize("level", [0, 6])
+@pytest.mark.parametrize("level", [-1, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9])
 def test_roundtrip_every_decoder(ctx, level):
     rng = random.Random(level)
     ps = [p[:65280] for p in payloads(rng)] + [b"x" * 17, bytes(range(256)) * 255]

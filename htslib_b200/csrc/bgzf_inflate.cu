@@ -473,20 +473,45 @@ __device__ uint32_t crc_finish(CrcCursor &c, uint32_t n)
 // issued before the current ones are first used (load_slot returns with its loads in flight), so a
 // round costs about one L2 round trip however many chunks it has: nothing a round stores is read
 // in that round.
-// Overlapping matches (dist < len, run-length style) are rare and take a separate cooperative
-// path with a per-byte modulo.
+// Overlapping matches (dist < len, run-length style) with dist <= 4 join the same word space: every
+// lane of such a match loads the one or two aligned words that hold its period [d0 - dist, d0)
+// (final before the round, by the dependency mask) and builds its destination word as the period
+// replicated and rotated to the word's phase.  On sorted BAM these are almost all dist == 1 runs in
+// the quality strings.  Longer periods take a cooperative path whose loads never wait on its stores.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t low_mask(uint32_t n) { return n >= 32u ? 0xffffffffu : (1u << n) - 1u; }
+
+constexpr uint32_t RUN_MAX_DIST = 4;     // overlapping matches up to this period are copied as words
+
+__device__ __forceinline__ uint32_t ld8_if(const uint8_t *a, bool c)
+{
+    uint32_t v;
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\tmov.u32 %0, 0;\n\t@q ld.global.u8 %0, [%1];\n\t}" : "=r"(v) : "l"(a), "r"((uint32_t)c) : "memory");
+    return v;
+}
 
 struct WordSlot {
     uint32_t d;               // destination word, from the aligned base
     uint32_t lo, hi;          // aligned source words (hi: 0 when the next lane's lo is meant)
     uint32_t f;               // [3:0] bytes of the word that belong to the match (0xf: all), [8:4] source shift,
-                              // [9] the upper source word is the next lane's lower one
+                              // [9] the upper source word is the next lane's lower one,
+                              // [10] run: the source word holds the period, [12:11] period - 1, [14:13] phase
 };
 
+// the word whose byte j is pat[(r + j) mod dist], pat = the low dist bytes of p (dist 1..4, r < dist)
+__device__ __forceinline__ uint32_t run_word(uint32_t p, uint32_t dist, uint32_t r)
+{
+    // lo:hi = the first 8 bytes of the periodic sequence
+    const uint32_t pat = p & low_mask(8u * dist);
+    const uint32_t lo = pat * (dist == 1u ? 0x01010101u : dist == 2u ? 0x00010001u : dist == 3u ? 0x01000001u : 1u);
+    const uint32_t hi = dist == 3u ? pat >> 8 | pat << 16 : lo;
+    return __funnelshift_r(lo, hi, 8u * r);
+}
+
 // word `slot` of the round's destination-word space.  inc: inclusive scan of the word counts;
-// wb = (first word of the lane's match) - 4 * (words in front of it); u0 = its destination; ld = len | dist << 16
+// wb = (first word of the lane's match) - 4 * (words in front of it); u0 = its destination; ld = len | dist << 16.
+// RUNS: the round has short-period runs (the run fields cost instructions on every word, so rounds without runs skip them)
+template <bool RUNS>
 __device__ __forceinline__ WordSlot load_slot(const uint8_t *ob, uint32_t inc, uint32_t wb, uint32_t u0, uint32_t ld,
                                               uint32_t slot, uint32_t T)
 {
@@ -500,26 +525,33 @@ __device__ __forceinline__ WordSlot load_slot(const uint8_t *ob, uint32_t inc, u
     const uint32_t kn = __shfl_down_sync(0xffffffffu, k, 1);
     const bool valid = slot < T;
     const uint32_t dist = l_d >> 16;
+    const bool run = RUNS && dist < (l_d & 0xffffu);                           // overlapping: dist <= RUN_MAX_DIST here
     const uint32_t a = max(D, a0), b = min(D + 4u, a0 + (l_d & 0xffffu));     // the match's bytes in this word
-    const int32_t S = (int32_t)(D - dist), S0 = S & ~3, sh = (S & 3) * 8;      // S >= -3: the source starts at >= 0
-    // only words that hold source bytes [a - dist, b - dist) are touched
-    const bool from_next = lane < 31 && kn == k && slot + 1 < T;               // the next lane's lower word is this one's upper
-    const bool need_lo = valid && S0 + 4 > (int32_t)(a - dist);
-    const bool need_hi = valid && sh != 0 && S0 + 4 < (int32_t)(b - dist) && !from_next;
+    // the source bytes this word needs: [a - dist, b - dist), or a run's whole period [a0 - dist, a0)
+    const uint32_t sa = run ? a0 - dist : a - dist, sb = run ? a0 : b - dist;
+    const int32_t S = (int32_t)(run ? a0 - dist : D - dist), S0 = S & ~3, sh = (S & 3) * 8;   // S >= -3: the source starts at >= 0
+    // only words that hold source bytes [sa, sb) are touched
+    const bool from_next = lane < 31 && kn == k && slot + 1 < T && !run;      // the next lane's lower word is this one's upper
+    const bool need_lo = valid && S0 + 4 > (int32_t)sa;
+    const bool need_hi = valid && sh != 0 && S0 + 4 < (int32_t)sb && !from_next;
     WordSlot w;
     w.d = D;
     w.lo = ld32_if(ob + S0, need_lo);
     w.hi = ld32_if(ob + S0 + 4, need_hi);
     const uint32_t m = valid ? ((1u << (b - D)) - 1u) & ~((1u << (a - D)) - 1u) : 0u;
-    w.f = m | (uint32_t)sh << 4 | (from_next ? 1u << 9 : 0u);
+    // a run's phase at D: (D - a0) mod dist, with D >= a0 - 3 and 12 a multiple of every period
+    const uint32_t t = D + 12u - a0, r = dist == 3u ? t % 3u : t & (dist - 1u);
+    w.f = m | (uint32_t)sh << 4 | (from_next ? 1u << 9 : 0u) | (run ? 1u << 10 | (dist - 1u) << 11 | r << 13 : 0u);
     return w;
 }
 
 // the first use of the loaded words: load_slot returns with its loads in flight
+template <bool RUNS>
 __device__ __forceinline__ void store_slot(uint8_t *ob, const WordSlot &w)
 {
     const uint32_t lo_next = __shfl_down_sync(0xffffffffu, w.lo, 1);
-    const uint32_t v = __funnelshift_r(w.lo, (w.f >> 9) ? lo_next : w.hi, (w.f >> 4) & 31u);
+    uint32_t v = __funnelshift_r(w.lo, ((w.f >> 9) & 1u) ? lo_next : w.hi, (w.f >> 4) & 31u);
+    if (RUNS && ((w.f >> 10) & 1u)) v = run_word(v, ((w.f >> 11) & 3u) + 1u, (w.f >> 13) & 3u);
     const uint32_t m = w.f & 15u;
     const bool part = m != 15u;
     st32_if(ob + w.d, v, !part);
@@ -527,6 +559,19 @@ __device__ __forceinline__ void store_slot(uint8_t *ob, const WordSlot &w)
     st8_if(ob + w.d + 1, v >> 8, part && (m & 2u));
     st8_if(ob + w.d + 2, v >> 16, part && (m & 4u));
     st8_if(ob + w.d + 3, v >> 24, part && (m & 8u));
+}
+
+// the round's T destination words, 32 at a time, the next 32 words' loads in flight while the current ones are stored
+template <bool RUNS>
+__device__ __forceinline__ void copy_words(uint8_t *ob, uint32_t inc, uint32_t wb, uint32_t u0, uint32_t ld, uint32_t T)
+{
+    WordSlot cur = load_slot<RUNS>(ob, inc, wb, u0, ld, hgpu_lane(), T);
+    for (uint32_t base = 0; base < T; base += 32) {
+        WordSlot nxt = {0u, 0u, 0u, 0u};
+        if (base + 32 < T) nxt = load_slot<RUNS>(ob, inc, wb, u0, ld, base + 32 + hgpu_lane(), T);
+        store_slot<RUNS>(ob, cur);
+        cur = nxt;
+    }
 }
 
 __device__ __forceinline__ void exec_batch(uint8_t *out, uint2 rec, uint32_t nrec)
@@ -555,7 +600,8 @@ __device__ __forceinline__ void exec_batch(uint8_t *out, uint2 rec, uint32_t nre
     const uint32_t mis = (uint32_t)reinterpret_cast<uintptr_t>(out) & 3u;
     uint8_t *ob = out - mis;
     const uint32_t u0 = dst + mis;
-    const uint32_t nw = have && !ov ? ((u0 + len + 3u) >> 2) - (u0 >> 2) : 0u;
+    const bool long_run = ov && dist > RUN_MAX_DIST;
+    const uint32_t nw = have && !long_run ? ((u0 + len + 3u) >> 2) - (u0 >> 2) : 0u;
     uint32_t done = low_mask(nrec) ^ 0xffffffffu;
 #ifdef HGPU_PROFILE
     if (lane == 0) atomicAdd(&g_prof[9], 1ull);
@@ -563,11 +609,13 @@ __device__ __forceinline__ void exec_batch(uint8_t *out, uint2 rec, uint32_t nre
     while (done != 0xffffffffu) {
         const bool ready = !((done >> lane) & 1u) && (dep & ~done) == 0u;
         const uint32_t R = __ballot_sync(0xffffffffu, ready);
-        const uint32_t Rov = __ballot_sync(0xffffffffu, ready && ov);
+        const uint32_t Rov = __ballot_sync(0xffffffffu, ready && long_run);
+        const bool runs = __any_sync(0xffffffffu, ready && ov && !long_run);
 #ifdef HGPU_PROFILE
-        if (lane == 0) { atomicAdd(&g_prof[8], 1ull); atomicAdd(&g_prof[11], (unsigned long long)__popc(Rov)); }
+        const uint32_t Rall = __ballot_sync(0xffffffffu, ready && ov);
+        if (lane == 0) { atomicAdd(&g_prof[8], 1ull); atomicAdd(&g_prof[11], (unsigned long long)__popc(Rall)); }
 #endif
-        // every ready match that does not overlap its own source: coalesced word copies
+        // every ready match except the long-period runs: coalesced word copies
         const uint32_t cnt = ready ? nw : 0u;
         uint32_t inc = cnt;
 #pragma unroll
@@ -578,29 +626,42 @@ __device__ __forceinline__ void exec_batch(uint8_t *out, uint2 rec, uint32_t nre
         const uint32_t T = __shfl_sync(0xffffffffu, inc, 31);
         const uint32_t wb = (u0 & ~3u) - 4u * (inc - cnt);
         if (T) {
-            WordSlot cur = load_slot(ob, inc, wb, u0, rec.y, lane, T);
-            for (uint32_t base = 0; base < T; base += 32) {
-                WordSlot nxt = {0u, 0u, 0u, 0u};
-                if (base + 32 < T) nxt = load_slot(ob, inc, wb, u0, rec.y, base + 32 + lane, T);
-                store_slot(ob, cur);
-                cur = nxt;
-            }
+            if (runs) copy_words<true>(ob, inc, wb, u0, rec.y, T);
+            else copy_words<false>(ob, inc, wb, u0, rec.y, T);
         }
         __syncwarp();
-        // overlapping matches of this round: the source is the `dist` bytes before the
-        // destination, repeated
+        // overlapping matches of this round with a period over RUN_MAX_DIST: byte i of the match is
+        // period byte i % dist.  The period lies in front of the destination and is never overwritten
+        // here, so no load waits on a store: a period of up to 32 bytes is loaded once (one byte per
+        // lane) and shuffled out, a longer one is loaded a step ahead of the stores that use it.
         for (uint32_t m = Rov; m; m &= m - 1) {
             const int k = __ffs(m) - 1;
             const uint32_t d0 = __shfl_sync(0xffffffffu, dst, k), ln = __shfl_sync(0xffffffffu, len, k);
             const uint32_t di = __shfl_sync(0xffffffffu, dist, k);
-            // i % di for i = lane, lane+32, ...: one division pair, then add-and-wrap.  The source bytes lie in
-            // front of the destination and are never overwritten here, so loads and stores need no phases.
+            const uint8_t *per = out + d0 - di;
+            // i % di for i = lane, lane+32, ...: one division pair, then add-and-wrap
             const uint32_t stepm = 32u % di;
             uint32_t r = lane % di;
-            for (uint32_t i = lane; i < ln; i += 32) {
-                out[d0 + i] = out[d0 - di + r];
-                r += stepm;
-                if (r >= di) r -= di;
+#ifdef HGPU_PROFILE
+            if (lane == 0) atomicAdd(&g_prof[14], (unsigned long long)((ln + 31u) / 32u));
+#endif
+            if (di <= 32u) {
+                const uint32_t pb = ld8_if(per + lane, lane < di);
+                for (uint32_t i = lane; i - lane < ln; i += 32) {
+                    const uint32_t v = __shfl_sync(0xffffffffu, pb, r);
+                    st8_if(out + d0 + i, v, i < ln);
+                    r += stepm;
+                    if (r >= di) r -= di;
+                }
+            } else {
+                uint32_t v = ld8_if(per + r, lane < ln);
+                for (uint32_t i = lane; i < ln; i += 32) {
+                    r += stepm;
+                    if (r >= di) r -= di;
+                    const uint32_t nv = ld8_if(per + r, i + 32u < ln);
+                    st8_if(out + d0 + i, v, true);
+                    v = nv;
+                }
             }
         }
         __syncwarp();                               // next round reads what other lanes just stored
@@ -660,7 +721,9 @@ __device__ int decode_body_uniform(InflateSmem &s, Bits &b, uint8_t *out, uint32
 // from a guessed start (the cut itself) to the end of its sub-range; Huffman streams
 // self-synchronise, so the position where lane i leaves its range is usually already the true
 // token boundary.  Each round lane i+1 restarts from lane i's exit if that moved; lane 0 is exact,
-// so after k rounds lanes 0..k are exact, and in practice two or three rounds settle all 32.
+// so after k rounds lanes 0..k are exact, and in practice two or three rounds settle all 32.  A
+// restarted lane stops as soon as it re-joins its round-0 path (checkpoints, below): on sorted BAM
+// that is a few tokens, not a second pass over the sub-range.
 // Then output offsets follow from a prefix sum of per-lane byte counts, a last pass writes the
 // literals and lists the matches, and the matches are executed in order through the window.
 // ---------------------------------------------------------------------------------------------
@@ -709,20 +772,67 @@ __device__ __forceinline__ uint32_t lb_lookup(const uint32_t *table, LaneBits &b
 
 enum : uint32_t { ST_RUN = 0, ST_EOB = 1, ST_BAD = 2 };
 
-// Decode tokens in [start, end).  EMIT=0: count output bytes / matches.  EMIT=1: write literals at
-// out[obase..] and {dst, len | dist<<16} match records at mrec[mbase..]; sets bad_dist on a
-// distance that reaches before the start of the output.
-template <int EMIT>
+// Round 0 of the re-sync records a checkpoint at every CK_STRIDE-th of the lane's first
+// CK_STRIDE * CK_TOKENS token boundaries: its bit position and the bytes and matches decoded in front
+// of it, plus round 0's result.  They live lane-interleaved (coalesced stores) in the warp's
+// match-record scratch, which is unused until the emit pass.  A later round that reaches one of
+// those positions is on round 0's path from there on (a token boundary determines everything decoded
+// after it), so it stops and takes round 0's remaining counts, exit and status.  Once the paths have
+// joined, the next checkpoint comes within CK_STRIDE tokens; a checkpoint at every token costs more
+// in round-0 stores than the earlier stop saves.
+constexpr uint32_t CK_TOKENS = 32;                     // checkpoints per lane
+constexpr uint32_t CK_STRIDE = 4;                      // tokens per checkpoint
+constexpr uint32_t CK_COUNTS = 32 * CK_TOKENS;         // ck[32 j]: position, ck[CK_COUNTS + 32 j]: bytes | matches << 16
+constexpr uint32_t CK_RESULT = 2 * CK_COUNTS;          // ck[CK_RESULT + 32 k]: round 0's exit, bytes, matches, status
+constexpr uint32_t CK_WORDS = CK_RESULT + 4 * 32;
+
+enum : int { LD_ROUND0 = 0, LD_EMIT = 1, LD_RESYNC = 2 };
+
+// Decode tokens in [start, end).  LD_ROUND0: count output bytes / matches, record the checkpoints at
+// ck (nck of them).  LD_RESYNC: the same, stopping where the path meets one of round 0's nck
+// checkpoints.  LD_EMIT: write literals at out[obase..] and {dst, len | dist<<16} match records at
+// mrec[mbase..]; sets bad_dist on a distance that reaches before the start of the output.
+// iters: loop iterations (tokens decoded).
+template <int MODE>
 __device__ __forceinline__ void lane_decode(const InflateSmem &s, const uint32_t *wbase, const uint32_t *wend,
                                             uint32_t start, uint32_t end, uint32_t &exitp, uint32_t &nout,
                                             uint32_t &nmatch, uint32_t &st, uint8_t *out, uint32_t obase,
-                                            uint2 *mrec, uint32_t mbase, bool &bad_dist)
+                                            uint2 *mrec, uint32_t mbase, bool &bad_dist,
+                                            uint32_t *ck, uint32_t &nck, uint32_t &iters)
 {
+    constexpr bool EMIT = MODE == LD_EMIT;
     LaneBits b;
-    uint32_t n = 0, m = 0, status = ST_RUN;
-    if (start >= end) { exitp = start; nout = 0; nmatch = 0; st = ST_RUN; return; }
+    uint32_t n = 0, m = 0, status = ST_RUN, it = 0;
+    if (MODE == LD_ROUND0) nck = 0;
+    if (start >= end) { exitp = start; nout = 0; nmatch = 0; st = ST_RUN; iters = 0; return; }
     lb_init(b, wbase, wend, start, end);
+    // LD_RESYNC: merge walk over the checkpoint positions, the next one in flight
+    const uint32_t *cp = ck, *cp_end = ck + 32 * (MODE == LD_RESYNC ? nck : 0u);
+    uint32_t cur = cp < cp_end ? cp[0] : 0xffffffffu;
+    uint32_t nxt = cp + 32 < cp_end ? cp[32] : 0xffffffffu;
     while (b.cnt > b.lim) {
+        if (MODE == LD_ROUND0 && it < CK_STRIDE * CK_TOKENS && it % CK_STRIDE == 0) {
+            ck[32 * (it / CK_STRIDE)] = lb_pos(b, end);
+            ck[CK_COUNTS + 32 * (it / CK_STRIDE)] = n | m << 16;
+        }
+        if (MODE == LD_RESYNC && cp < cp_end) {
+            const uint32_t p = lb_pos(b, end);
+            while (cur < p && cp < cp_end) {
+                cp += 32;
+                cur = nxt;
+                nxt = cp + 32 < cp_end ? cp[32] : 0xffffffffu;
+            }
+            if (cur == p) {                    // on round 0's path from here
+                const uint32_t c = cp[CK_COUNTS];
+                exitp = ck[CK_RESULT];
+                nout = n + ck[CK_RESULT + 32] - (c & 0xffffu);
+                nmatch = m + ck[CK_RESULT + 64] - (c >> 16);
+                st = ck[CK_RESULT + 96];
+                iters = it;
+                return;
+            }
+        }
+        it++;
         lb_fill(b, wend);
         uint32_t e = lb_lookup<LIT_ROOT>(s.lit, b);
         uint32_t kind = (e >> 4) & 15;
@@ -750,6 +860,11 @@ __device__ __forceinline__ void lane_decode(const InflateSmem &s, const uint32_t
     }
     exitp = lb_pos(b, end);
     nout = n; nmatch = m; st = status;
+    iters = it;
+    if (MODE == LD_ROUND0) {
+        nck = min((it + CK_STRIDE - 1) / CK_STRIDE, CK_TOKENS);
+        ck[CK_RESULT] = exitp; ck[CK_RESULT + 32] = n; ck[CK_RESULT + 64] = m; ck[CK_RESULT + 96] = status;
+    }
 }
 
 // Execute mrec[0..total) in order through the window.  Records are fetched 32 at a time
@@ -771,6 +886,7 @@ __device__ void run_matches(uint8_t *out, const uint2 *mrec, uint32_t total, Crc
 
 constexpr uint32_t PAR_MIN_BITS = 32 * 96;      // below this a deflate block is decoded serially
 constexpr uint32_t MREC_CAP = 65536 / 3 + 64;   // a match yields >= 3 bytes of a <= 64 KiB member
+static_assert(CK_WORDS <= 2 * MREC_CAP, "the re-sync checkpoints fit the match-record scratch");
 
 // Parallel decode of one Huffman block body starting at bit `body` of the member (bit 0 = first
 // bit of word wbase[0], i.e. positions include the alignment offset).  total = end of input.
@@ -783,10 +899,21 @@ __device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const
     uint32_t start = body + lane * S;
     uint32_t end = lane == 31 ? total : min(total, body + (lane + 1) * S);
     if (start > total) start = total;
-    uint32_t exitp = 0, n = 0, m = 0, st = ST_RUN;
+    uint32_t exitp = 0, n = 0, m = 0, st = ST_RUN, iters = 0;
     bool need = true, dummy = false;
+    uint32_t nck = 0;
+    uint32_t *ck = reinterpret_cast<uint32_t *>(mrec) + lane;     // round 0's checkpoints (CK_WORDS <= 2 * mcap)
     for (int round = 0; round < 34; round++) {
-        if (need) lane_decode<0>(s, wbase, wend, start, end, exitp, n, m, st, nullptr, 0, nullptr, 0, dummy);
+        if (round == 0)
+            lane_decode<LD_ROUND0>(s, wbase, wend, start, end, exitp, n, m, st, nullptr, 0, nullptr, 0, dummy, ck, nck, iters);
+        else if (need)
+            lane_decode<LD_RESYNC>(s, wbase, wend, start, end, exitp, n, m, st, nullptr, 0, nullptr, 0, dummy, ck, nck, iters);
+        else
+            iters = 0;
+#ifdef HGPU_PROFILE
+        const uint32_t wi = __reduce_max_sync(0xffffffffu, iters);       // the warp's loop iterations this round
+        if (lane == 0) atomicAdd(&g_prof[round == 0 ? 12 : 13], (unsigned long long)wi);
+#endif
         uint32_t prev = __shfl_up_sync(0xffffffffu, exitp, 1);
         uint32_t ns = lane == 0 ? start : prev;
         need = ns != start;
@@ -816,7 +943,7 @@ __device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const
     bool bad_dist = false;
     if (lane <= E) {
         uint32_t e2, n2, m2, st2;
-        lane_decode<1>(s, wbase, wend, start, end, e2, n2, m2, st2, out, o + on - n, mrec, mn - m, bad_dist);
+        lane_decode<LD_EMIT>(s, wbase, wend, start, end, e2, n2, m2, st2, out, o + on - n, mrec, mn - m, bad_dist, ck, nck, iters);
     }
     if (__any_sync(0xffffffffu, bad_dist)) return HGPU_BGZF_ERR_ZLIB;   // distance too far back
     __syncwarp();
@@ -1033,6 +1160,7 @@ bgzf_inflate_kernel(const uint8_t *__restrict__ in, const uint64_t *__restrict__
 // library); CRAM writes its GZIP blocks with memLevel 9 (cram_io.c zlib_mem_deflate): at most 32 767 symbols per block.
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t GZ_MREC = 32768 + 64;
+static_assert(CK_WORDS <= 2 * GZ_MREC, "the re-sync checkpoints fit the match-record scratch");
 
 __device__ int gzip_header_len(const uint8_t *h, uint32_t n)
 {

@@ -25,3 +25,10 @@ with torch.cuda.stream(s):
         ms=e0.elapsed_time(e1)
         ok = L.hgpu_debug_profile(buf)
         print(quals, "ms", round(ms,3), "GB/s", round(float(ulen.sum())/ms/1e6,1), "errors", int(d_st.abs().sum()), "prof(cycles/block):", [int(x)//nb for x in buf] if ok==0 else None)
+        if ok == 0:
+            # counters per block: exec_batch rounds and batches, overlapping matches, the warp's Huffman loop iterations
+            # in re-sync round 0 and in the later rounds (warp max per round, summed), iterations of the long-period run path
+            per = lambda i: round(int(buf[i]) / nb, 1)
+            r0 = per(12)
+            print("  rounds", per(8), "batches", per(9), "overlapping", per(11), "resync: round 0", r0, "later rounds", per(13),
+                  "(x%.2f of one pass)" % ((r0 + per(13)) / r0 if r0 else 0.0), "long-period run iterations", per(14))

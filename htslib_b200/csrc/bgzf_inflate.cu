@@ -47,6 +47,8 @@ struct InflateSmem {
         };
         struct {                     // match execution
             uint2 rbuf[32];          // match records parked by the serial decoder
+            uint2 own[32];           // a round's word-copy matches in slot order: {first word - 4 * first slot, destination}
+            uint32_t own_ld[32];     // and their len | dist << 16
         };
     };
 };
@@ -347,10 +349,6 @@ __device__ __forceinline__ uint32_t ld32_if(const uint8_t *a, bool c)
     asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\tmov.u32 %0, 0;\n\t@q ld.global.u32 %0, [%1];\n\t}" : "=r"(v) : "l"(a), "r"((uint32_t)c) : "memory");
     return v;
 }
-__device__ __forceinline__ void st32_if(uint8_t *a, uint32_t v, bool c)
-{
-    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.global.u32 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"((uint32_t)c) : "memory");
-}
 __device__ __forceinline__ void st8_if(uint8_t *a, uint32_t v, bool c)
 {
     asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.global.u8 [%0], %1;\n\t}" :: "l"(a), "r"(v), "r"((uint32_t)c) : "memory");
@@ -466,8 +464,11 @@ __device__ uint32_t crc_finish(CrcCursor &c, uint32_t n)
 // A round's ready matches that do not overlap their own source are laid end to end in one space
 // of destination words (4-byte aligned words that hold at least one byte of the match; an
 // exclusive scan of the per-match word counts), and the warp walks that space 32 words at a time:
-// lane j finds its match by a 5-step search over the inclusive scan, funnel-shifts the word from
-// the aligned source words in front of it (the upper one is usually the next lane's lower one)
+// the round's matches are listed once, in slot order, in a small table in shared memory, and lane j
+// finds its match there from a 32-bit mask of the slots where a match starts (one reduction, a popc
+// and one shared load instead of a 5-step shuffle search and four broadcasts per 32 words), funnel-
+// shifts the word from the aligned source words in front of it (the upper one is usually the next
+// lane's lower one)
 // and stores it whole, or bytewise where the word is shared with a literal or another match.
 // Lanes on one match touch the same one or two cache lines.  The loads of the next 32 words are
 // issued before the current ones are first used (load_slot returns with its loads in flight), so a
@@ -508,21 +509,17 @@ __device__ __forceinline__ uint32_t run_word(uint32_t p, uint32_t dist, uint32_t
     return __funnelshift_r(lo, hi, 8u * r);
 }
 
-// word `slot` of the round's destination-word space.  inc: inclusive scan of the word counts;
-// wb = (first word of the lane's match) - 4 * (words in front of it); u0 = its destination; ld = len | dist << 16.
+// word `slot` of the round's destination-word space.  The round's matches are s.own / s.own_ld in slot order;
+// carry: the matches that start in front of this chunk, sm: bit j set where a match starts at the chunk's slot j.
 // RUNS: the round has short-period runs (the run fields cost instructions on every word, so rounds without runs skip them)
 template <bool RUNS>
-__device__ __forceinline__ WordSlot load_slot(const uint8_t *ob, uint32_t inc, uint32_t wb, uint32_t u0, uint32_t ld,
+__device__ __forceinline__ WordSlot load_slot(const uint8_t *ob, const InflateSmem &s, uint32_t carry, uint32_t sm,
                                               uint32_t slot, uint32_t T)
 {
     const uint32_t lane = hgpu_lane();
-    uint32_t k = 0;                                            // owner: the number of matches ending at or before slot
-#pragma unroll
-    for (int st = 16; st >= 1; st >>= 1)
-        if (__shfl_sync(0xffffffffu, inc, k + st - 1) <= slot) k += st;
-    const uint32_t D = __shfl_sync(0xffffffffu, wb, k) + 4u * slot;
-    const uint32_t a0 = __shfl_sync(0xffffffffu, u0, k), l_d = __shfl_sync(0xffffffffu, ld, k);
-    const uint32_t kn = __shfl_down_sync(0xffffffffu, k, 1);
+    const uint32_t k = carry + __popc(sm & ((2u << lane) - 1u)) - 1u;     // owner: the last match starting at or before slot
+    const uint2 own = s.own[k];
+    const uint32_t D = own.x + 4u * slot, a0 = own.y, l_d = s.own_ld[k];
     const bool valid = slot < T;
     const uint32_t dist = l_d >> 16;
     const bool run = RUNS && dist < (l_d & 0xffffu);                           // overlapping: dist <= RUN_MAX_DIST here
@@ -531,7 +528,7 @@ __device__ __forceinline__ WordSlot load_slot(const uint8_t *ob, uint32_t inc, u
     const uint32_t sa = run ? a0 - dist : a - dist, sb = run ? a0 : b - dist;
     const int32_t S = (int32_t)(run ? a0 - dist : D - dist), S0 = S & ~3, sh = (S & 3) * 8;   // S >= -3: the source starts at >= 0
     // only words that hold source bytes [sa, sb) are touched
-    const bool from_next = lane < 31 && kn == k && slot + 1 < T && !run;      // the next lane's lower word is this one's upper
+    const bool from_next = lane < 31 && !((sm >> lane) & 2u) && slot + 1 < T && !run;   // the next lane's lower word is this one's upper
     const bool need_lo = valid && S0 + 4 > (int32_t)sa;
     const bool need_hi = valid && sh != 0 && S0 + 4 < (int32_t)sb && !from_next;
     WordSlot w;
@@ -552,29 +549,45 @@ __device__ __forceinline__ void store_slot(uint8_t *ob, const WordSlot &w)
     const uint32_t lo_next = __shfl_down_sync(0xffffffffu, w.lo, 1);
     uint32_t v = __funnelshift_r(w.lo, ((w.f >> 9) & 1u) ? lo_next : w.hi, (w.f >> 4) & 31u);
     if (RUNS && ((w.f >> 10) & 1u)) v = run_word(v, ((w.f >> 11) & 3u) + 1u, (w.f >> 13) & 3u);
-    const uint32_t m = w.f & 15u;
-    const bool part = m != 15u;
-    st32_if(ob + w.d, v, !part);
-    st8_if(ob + w.d, v, part && (m & 1u));
-    st8_if(ob + w.d + 1, v >> 8, part && (m & 2u));
-    st8_if(ob + w.d + 2, v >> 16, part && (m & 4u));
-    st8_if(ob + w.d + 3, v >> 24, part && (m & 8u));
+    // the whole word, or the bytes of mask m (w.f & 15) one by one: one predicate per byte, taken from the mask
+    // inside one asm block (2 % off the kernel against predicates built from C++ booleans, one asm store each)
+    asm volatile("{\n\t.reg .pred pw, p0, p1, p2, p3;\n\t.reg .b32 m, t;\n\t"
+                 "and.b32 m, %2, 15;\n\t"
+                 "setp.eq.u32 pw, m, 15;\n\t"
+                 "@pw st.global.u32 [%0], %1;\n\t"
+                 "selp.b32 m, 0, m, pw;\n\t"
+                 "and.b32 t, m, 1;\n\tsetp.ne.u32 p0, t, 0;\n\t"
+                 "and.b32 t, m, 2;\n\tsetp.ne.u32 p1, t, 0;\n\t"
+                 "and.b32 t, m, 4;\n\tsetp.ne.u32 p2, t, 0;\n\t"
+                 "and.b32 t, m, 8;\n\tsetp.ne.u32 p3, t, 0;\n\t"
+                 "@p0 st.global.u8 [%0], %1;\n\t"
+                 "shr.b32 t, %1, 8;\n\t@p1 st.global.u8 [%0+1], t;\n\t"
+                 "shr.b32 t, %1, 16;\n\t@p2 st.global.u8 [%0+2], t;\n\t"
+                 "shr.b32 t, %1, 24;\n\t@p3 st.global.u8 [%0+3], t;\n\t}"
+                 :: "l"(ob + w.d), "r"(v), "r"(w.f) : "memory");
 }
 
-// the round's T destination words, 32 at a time, the next 32 words' loads in flight while the current ones are stored
+// the round's T destination words, 32 at a time, the next 32 words' loads in flight while the current ones are stored.
+// The lane's match (if cnt, its word count, is not 0) starts at slot ex.
 template <bool RUNS>
-__device__ __forceinline__ void copy_words(uint8_t *ob, uint32_t inc, uint32_t wb, uint32_t u0, uint32_t ld, uint32_t T)
+__device__ __forceinline__ void copy_words(uint8_t *ob, const InflateSmem &s, uint32_t ex, uint32_t cnt, uint32_t T)
 {
-    WordSlot cur = load_slot<RUNS>(ob, inc, wb, u0, ld, hgpu_lane(), T);
+    const auto starts = [&](uint32_t base) { return __reduce_or_sync(0xffffffffu, cnt && ex - base < 32u ? 1u << (ex - base) : 0u); };
+    uint32_t sm = starts(0), carry = 0;
+    WordSlot cur = load_slot<RUNS>(ob, s, carry, sm, hgpu_lane(), T);
     for (uint32_t base = 0; base < T; base += 32) {
         WordSlot nxt = {0u, 0u, 0u, 0u};
-        if (base + 32 < T) nxt = load_slot<RUNS>(ob, inc, wb, u0, ld, base + 32 + hgpu_lane(), T);
+        if (base + 32 < T) {
+            carry += __popc(sm);
+            sm = starts(base + 32);
+            nxt = load_slot<RUNS>(ob, s, carry, sm, base + 32 + hgpu_lane(), T);
+        }
         store_slot<RUNS>(ob, cur);
         cur = nxt;
     }
 }
 
-__device__ __forceinline__ void exec_batch(uint8_t *out, uint2 rec, uint32_t nrec)
+__device__ __forceinline__ void exec_batch(InflateSmem &s, uint8_t *out, uint2 rec, uint32_t nrec)
 {
     const uint32_t lane = hgpu_lane();
     const bool have = lane < nrec;
@@ -624,10 +637,17 @@ __device__ __forceinline__ void exec_batch(uint8_t *out, uint2 rec, uint32_t nre
             if (lane >= (uint32_t)d) inc += t;
         }
         const uint32_t T = __shfl_sync(0xffffffffu, inc, 31);
-        const uint32_t wb = (u0 & ~3u) - 4u * (inc - cnt);
         if (T) {
-            if (runs) copy_words<true>(ob, inc, wb, u0, rec.y, T);
-            else copy_words<false>(ob, inc, wb, u0, rec.y, T);
+            // the owner table: the matches with words, in slot order
+            const uint32_t ex = inc - cnt, W = __ballot_sync(0xffffffffu, cnt != 0u);
+            if (cnt) {
+                const uint32_t k = __popc(W & hgpu_lanemask_lt());
+                s.own[k] = make_uint2((u0 & ~3u) - 4u * ex, u0);
+                s.own_ld[k] = rec.y;
+            }
+            __syncwarp();
+            if (runs) copy_words<true>(ob, s, ex, cnt, T);
+            else copy_words<false>(ob, s, ex, cnt, T);
         }
         __syncwarp();
         // overlapping matches of this round with a period over RUN_MAX_DIST: byte i of the match is
@@ -702,13 +722,13 @@ __device__ int decode_body_uniform(InflateSmem &s, Bits &b, uint8_t *out, uint32
         o += len;
         if (++pend == 32) {
             __syncwarp();
-            exec_batch(out, s.rbuf[lane], 32);
+            exec_batch(s, out, s.rbuf[lane], 32);
             pend = 0;
             crc_advance(crc, o);                           // literals are stored as they are decoded: all of [0, o) is final
         }
     }
     __syncwarp();
-    if (pend) exec_batch(out, s.rbuf[lane], pend);
+    if (pend) exec_batch(s, out, s.rbuf[lane], pend);
     __syncwarp();
     if (bits_overrun(b)) return HGPU_BGZF_ERR_ZLIB;
     return HGPU_OK;
@@ -871,14 +891,14 @@ __device__ __forceinline__ void lane_decode(const InflateSmem &s, const uint32_t
 // (coalesced) and broadcast with shuffles, so every lane sees the same match.
 // After a batch every byte in front of the next batch's first destination is final (literals were
 // written by the emit pass, earlier matches are done): the CRC cursor takes it.
-__device__ void run_matches(uint8_t *out, const uint2 *mrec, uint32_t total, CrcCursor &crc)
+__device__ void run_matches(InflateSmem &s, uint8_t *out, const uint2 *mrec, uint32_t total, CrcCursor &crc)
 {
     const uint32_t lane = hgpu_lane();
     uint2 nx = lane < total ? mrec[lane] : make_uint2(0, 0);
     for (uint32_t base = 0; base < total; base += 32) {
         uint2 rec = nx;
         nx = base + 32 + lane < total ? mrec[base + 32 + lane] : make_uint2(0, 0);      // next batch in flight
-        exec_batch(out, rec, total - base < 32u ? total - base : 32u);
+        exec_batch(s, out, rec, total - base < 32u ? total - base : 32u);
         if (base + 32 < total) crc_advance(crc, __shfl_sync(0xffffffffu, nx.x, 0));
     }
     __syncwarp();
@@ -949,7 +969,7 @@ __device__ int decode_body_parallel(InflateSmem &s, const uint32_t *wbase, const
     __syncwarp();
     __threadfence_block();
     pf.mark(2);
-    run_matches(out, mrec, tot_m, crc);
+    run_matches(s, out, mrec, tot_m, crc);
     pf.mark(3);
     o += tot_out;
     end_pos = last;

@@ -3,11 +3,14 @@
     python tools/inflate_shape.py [--blocks 40] [--quals novaseq|hiseq] [--level 6]
 
 For each BGZF block it decodes the token stream with a plain Python inflater and prints: tokens, matches,
-match batches (32 records) and the exec_batch rounds the dependency levels give, the overlapping matches
+match batches (32 records); rounds and 32-word copy chunks for two schedules of the match records: batches of 32
+run to completion (the kernel's exec_batch) and a rolling window of the 32 oldest pending records refilled every
+round (DESIGN.md §6 has its measurement); a round executes every record whose sources are final; the overlapping matches
 (dist < len) by distance and length, and the lane-parallel re-sync: the warp maximum of tokens a lane decodes
 in round 0, in round 1 when it re-decodes its whole sub-range, and in round 1 when it stops where it meets
 its round-0 path (the kernel's checkpoints)."""
 import argparse
+import bisect
 import os
 import sys
 import zlib
@@ -23,7 +26,7 @@ LX = [0] * 8 + [1] * 4 + [2] * 4 + [3] * 4 + [4] * 4 + [5] * 4 + [0]
 DB = [1, 2, 3, 4, 5, 7, 9, 13, 17, 25, 33, 49, 65, 97, 129, 193, 257, 385, 513, 769, 1025, 1537, 2049, 3073, 4097, 6145,
       8193, 12289, 16385, 24577]
 DX = [0, 0, 0, 0] + [k // 2 for k in range(2, 28)]
-PAR_MIN_BITS, LANES = 32 * 96, 32
+PAR_MIN_BITS, LANES, RUN_MAX_DIST = 32 * 96, 32, 4
 
 
 class Bits:
@@ -111,16 +114,47 @@ def block_shape(raw):
             return v, len(raw) * 8 + 64, toks, bodies          # the kernel's input end includes the 8-byte footer
 
 
+def deps(ms):
+    """per match, the index range [a, b) of the earlier matches whose destination overlaps its source"""
+    ds, es = [m[0] for m in ms], [m[0] + m[1] for m in ms]
+    out = []
+    for d, ln, di in ms:
+        s, e = d - di, d if di < ln else d - di + ln
+        out.append((bisect.bisect_right(es, s), bisect.bisect_left(ds, e)))
+    return out
+
+
+def words(m):
+    """destination words of a match in the round's word copy (output aligned to 4 bytes); long-period runs take none"""
+    d, ln, di = m
+    return 0 if RUN_MAX_DIST < di < ln else (d + ln + 3) // 4 - d // 4
+
+
 def rounds(ms):
-    """exec_batch rounds: per batch of 32 records, the depth of the dependency levels"""
-    total = 0
+    """batches of 32 records, each run to completion: (rounds, 32-word copy chunks)"""
+    dep, rs, ch = deps(ms), 0, 0
     for i in range(0, len(ms), 32):
-        B, lvl = ms[i:i + 32], []
-        for j, (d, ln, di) in enumerate(B):
-            s, e = d - di, d if di < ln else d - di + ln
-            lvl.append(1 + max([lvl[q] for q in range(j) if B[q][0] < e and B[q][0] + B[q][1] > s], default=0))
-        total += max(lvl)
-    return total
+        lvl = {}
+        for j in range(i, min(i + 32, len(ms))):
+            a, b = dep[j]
+            lvl[j] = 1 + max([lvl[q] for q in range(max(a, i), b)], default=0)
+        for r in range(1, max(lvl.values()) + 1):
+            ch += -(-sum(words(ms[j]) for j, v in lvl.items() if v == r) // 32)
+        rs += max(lvl.values())
+    return rs, ch
+
+
+def window_rounds(ms, W=32):
+    """rolling window of the W oldest pending records, refilled every round: (rounds, 32-word copy chunks)"""
+    dep, done, pend, rs, ch = deps(ms), [False] * len(ms), list(range(len(ms))), 0, 0
+    while pend:
+        ready = [j for j in pend[:W] if all(done[q] for q in range(*dep[j]))]
+        for j in ready:
+            done[j] = True
+        ch += -(-sum(words(ms[j]) for j in ready) // 32)
+        pend = [j for j in pend if not done[j]]
+        rs += 1
+    return rs, ch
 
 
 def resync(v, total, body, lt, dt):
@@ -150,7 +184,7 @@ def main():
     c = synth.bam_bgzf_corpus(3e6, level=args.level, quals=args.quals, procs=1)
     comp, clen = c["comp"], c["clen"]
     off, rows, ov = 0, [], []
-    print("block tokens matches batches rounds overlapping resync_r0 resync_r1_full resync_r1_converged")
+    print("block tokens matches batches rounds chunks window_rounds window_chunks overlapping resync_r0 resync_r1_full resync_r1_converged")
     for k in range(min(args.blocks, len(clen))):
         blk = bytes(comp[off:off + int(clen[k])]); off += int(clen[k])
         v, total, toks, bodies = block_shape(blk[18:-8])
@@ -159,7 +193,7 @@ def main():
         ov += o
         body, lt, dt = bodies[0]
         rs = resync(v, total, body, lt, dt) if total - body >= PAR_MIN_BITS else (0, 0, 0)
-        rows.append((len(toks), len(ms), (len(ms) + 31) // 32, rounds(ms), len(o)) + rs)
+        rows.append((len(toks), len(ms), (len(ms) + 31) // 32) + rounds(ms) + window_rounds(ms) + (len(o),) + rs)
         print(k, *rows[-1])
     a = np.array(rows, dtype=np.float64).mean(axis=0)
     print("mean", " ".join("%.1f" % x for x in a))

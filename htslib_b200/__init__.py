@@ -14,6 +14,8 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "htsgpu.h")
 HGPU_OK = 0
 BGZF_ERR_ZLIB, BGZF_ERR_CRC, BGZF_ERR_HEADER, BGZF_ERR_SPACE = -1, -2, -3, -4
 RANS_ERR = -1
+ERR_ARG = -102
+IDX_ERR_READ, IDX_ERR_PUSH = -10, -11
 
 _lib = None
 u8p = C.POINTER(C.c_uint8)
@@ -313,6 +315,33 @@ class Context:
         rc = lib().hgpu_bgzf_inflate_file_host(self.h, file_np.ctypes.data, file_np.size, out_np.ctypes.data, out_np.size,
                                                C.byref(out_len), C.byref(bad))
         return rc, out_len.value, bad.value
+
+    def bam_index(self, file_np, min_shift=0, window_bytes=0):
+        """The BAI (min_shift <= 0) or CSI (min_shift > 0) file of a whole BAM image, as sam_index_build3 writes it
+        (hgpu_bam_index_build_host).  Raises HgpuError with .code and .bad (the refused record, or the bad block)."""
+        L = lib()
+        L.hgpu_bam_index_build_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_uint64,
+                                                C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_int64)]
+        L.hgpu_bam_index_build_host.restype = C.c_int
+        out, n, bad = C.c_void_p(), C.c_uint64(0), C.c_int64(-1)
+        rc = L.hgpu_bam_index_build_host(self.h, file_np.ctypes.data, file_np.size, min_shift, window_bytes,
+                                         C.byref(out), C.byref(n), C.byref(bad))
+        if rc != HGPU_OK:
+            e = HgpuError("bam_index failed: rc=%d bad=%d (%s)" % (rc, bad.value, last_error()))
+            e.code, e.bad = rc, bad.value
+            raise e
+        try:
+            return C.string_at(out, n.value)
+        finally:
+            libc = C.CDLL(None)
+            libc.free.argtypes = [C.c_void_p]
+            libc.free(out)
+
+    def bam_index_last_ms(self):
+        """(device ms of the windows, host finishing ms) of the last bam_index call."""
+        ms = (C.c_float * 2)()
+        lib().hgpu_bam_index_last_ms(ms)
+        return ms[0], ms[1]
 
     def rans_nx16_decode_host(self, in_np, in_off, in_len, out_np, out_off, out_len):
         import numpy as np

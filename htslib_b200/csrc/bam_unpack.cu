@@ -24,15 +24,17 @@ __device__ __forceinline__ uint32_t ld32(const uint8_t *p)
     return p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24;
 }
 
-// walk records from `pos` while pos < end; returns count (or BROKEN) and the exit position
+// walk records from `pos` while pos < end; returns count (or BROKEN) and the exit position.  open: the stream is a
+// window of a longer one, so a record that runs past len ends the walk there (exitp = its start) instead of breaking it.
 __device__ uint64_t walk(const uint8_t *st, uint64_t len, uint64_t pos, uint64_t end, uint64_t &exitp,
-                         uint64_t *emit, uint64_t emit_cap, uint64_t emit_base)
+                         uint64_t *emit, uint64_t emit_cap, uint64_t emit_base, bool open = false)
 {
     uint64_t n = 0;
     while (pos < end) {
-        if (len - pos < 4) { exitp = pos; return BROKEN; }
+        if (len - pos < 4) { exitp = pos; return open ? n : BROKEN; }
         int32_t bl = (int32_t)ld32(st + pos);
-        if (bl < 32 || pos + 4 + (uint64_t)bl > len) { exitp = pos; return BROKEN; }
+        if (bl < 32) { exitp = pos; return BROKEN; }
+        if (pos + 4 + (uint64_t)bl > len) { exitp = pos; return open ? n : BROKEN; }
         if (emit && emit_base + n < emit_cap) emit[emit_base + n] = pos;
         n++;
         pos += 4 + (uint64_t)bl;
@@ -42,7 +44,7 @@ __device__ uint64_t walk(const uint8_t *st, uint64_t len, uint64_t pos, uint64_t
 }
 
 __global__ void bam_seg_scan_kernel(const uint8_t *st, uint64_t len, const uint64_t *hint, uint64_t nseg,
-                                    uint64_t *seg_start, uint64_t *seg_cnt, uint64_t *seg_exit)
+                                    uint64_t *seg_start, uint64_t *seg_cnt, uint64_t *seg_exit, bool open)
 {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= nseg) return;
@@ -51,14 +53,14 @@ __global__ void bam_seg_scan_kernel(const uint8_t *st, uint64_t len, const uint6
     if (e > len) e = len;
     uint64_t ex;
     seg_start[i] = s;
-    seg_cnt[i] = walk(st, len, s, e, ex, nullptr, 0, 0);
+    seg_cnt[i] = walk(st, len, s, e, ex, nullptr, 0, 0, open);
     seg_exit[i] = ex;
 }
 
 // single CTA: make the chain consistent, then exclusive-scan the counts
 __global__ void __launch_bounds__(1024)
 bam_seg_fix_kernel(const uint8_t *st, uint64_t len, const uint64_t *hint, uint64_t nseg, uint64_t *seg_start,
-                   uint64_t *seg_cnt, uint64_t *seg_exit, uint64_t *seg_base, uint64_t *n_rec)
+                   uint64_t *seg_cnt, uint64_t *seg_exit, uint64_t *seg_base, uint64_t *n_rec, bool open, uint64_t *tail)
 {
     __shared__ uint64_t part[1024];
     __shared__ int again;
@@ -81,7 +83,7 @@ bam_seg_fix_kernel(const uint8_t *st, uint64_t len, const uint64_t *hint, uint64
                 uint64_t e = i + 1 < nseg ? hint[i + 1] : len, ex;
                 if (e > len) e = len;
                 seg_start[i] = want;
-                seg_cnt[i] = walk(st, len, want, e, ex, nullptr, 0, 0);
+                seg_cnt[i] = walk(st, len, want, e, ex, nullptr, 0, 0, open);
                 seg_exit[i] = ex;
                 again = 1;
             }
@@ -102,6 +104,7 @@ bam_seg_fix_kernel(const uint8_t *st, uint64_t len, const uint64_t *hint, uint64
         uint64_t run = 0;
         for (int k = 0; k < 1024; k++) { uint64_t v = part[k]; part[k] = run; run += v; }
         *n_rec = run;
+        if (tail) *tail = seg_exit[nseg - 1];
     }
     __syncthreads();
     uint64_t run = part[t];
@@ -311,24 +314,38 @@ bam_unpack_kernel(const uint8_t *st, const uint64_t *rec_off, uint64_t n, hgpu_b
 
 } // namespace
 
-extern "C" int hgpu_bam_index_records_dev(hgpu_ctx *ctx, const uint8_t *d_stream, uint64_t len,
-                                          const uint64_t *d_hint_off, uint64_t n_hint, uint64_t *d_rec_off,
-                                          uint64_t rec_cap, uint64_t *d_n_rec, void *stream)
+static int bam_records(hgpu_ctx *ctx, const uint8_t *d_stream, uint64_t len, const uint64_t *d_hint_off, uint64_t n_hint,
+                       uint64_t *d_rec_off, uint64_t rec_cap, uint64_t *d_n_rec, uint64_t *d_tail, cudaStream_t st)
 {
-    if (!ctx || !d_stream || !d_n_rec) { hgpu_set_error("bad argument"); return HGPU_ERR_ARG; }
-    cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
+    const bool open = d_tail != nullptr;
     uint64_t nseg = d_hint_off && n_hint ? n_hint : 1;
     int rc = hgpu_ensure_bam(ctx, nseg * 4 * sizeof(uint64_t));
     if (rc) return rc;
     uint64_t *seg_start = (uint64_t *)ctx->d_bam, *seg_cnt = seg_start + nseg, *seg_exit = seg_cnt + nseg, *seg_base = seg_exit + nseg;
     const uint64_t *hint = nseg > 1 || (d_hint_off && n_hint) ? d_hint_off : nullptr;
     unsigned blocks = (unsigned)((nseg + 127) / 128);
-    bam_seg_scan_kernel<<<blocks, 128, 0, st>>>(d_stream, len, hint, nseg, seg_start, seg_cnt, seg_exit);
-    bam_seg_fix_kernel<<<1, 1024, 0, st>>>(d_stream, len, hint, nseg, seg_start, seg_cnt, seg_exit, seg_base, d_n_rec);
+    bam_seg_scan_kernel<<<blocks, 128, 0, st>>>(d_stream, len, hint, nseg, seg_start, seg_cnt, seg_exit, open);
+    bam_seg_fix_kernel<<<1, 1024, 0, st>>>(d_stream, len, hint, nseg, seg_start, seg_cnt, seg_exit, seg_base, d_n_rec, open, d_tail);
     if (d_rec_off)
         bam_seg_emit_kernel<<<blocks, 128, 0, st>>>(d_stream, len, hint, nseg, seg_start, seg_base, d_rec_off, rec_cap);
     hgpu_count_launch(d_rec_off ? 3 : 2);
     return hgpu_check(cudaGetLastError(), "bam index launch");
+}
+
+extern "C" int hgpu_bam_index_records_dev(hgpu_ctx *ctx, const uint8_t *d_stream, uint64_t len,
+                                          const uint64_t *d_hint_off, uint64_t n_hint, uint64_t *d_rec_off,
+                                          uint64_t rec_cap, uint64_t *d_n_rec, void *stream)
+{
+    if (!ctx || !d_stream || !d_n_rec) { hgpu_set_error("bad argument"); return HGPU_ERR_ARG; }
+    return bam_records(ctx, d_stream, len, d_hint_off, n_hint, d_rec_off, rec_cap, d_n_rec, nullptr,
+                       stream ? (cudaStream_t)stream : ctx->stream);
+}
+
+int hgpu_bam_records_window_dev(hgpu_ctx *ctx, const uint8_t *d_stream, uint64_t len, const uint64_t *d_hint_off,
+                                uint64_t n_hint, uint64_t *d_rec_off, uint64_t rec_cap, uint64_t *d_n_rec, uint64_t *d_tail,
+                                cudaStream_t st)
+{
+    return bam_records(ctx, d_stream, len, d_hint_off, n_hint, d_rec_off, rec_cap, d_n_rec, d_tail, st);
 }
 
 extern "C" int hgpu_bam_layout_dev(hgpu_ctx *ctx, const uint8_t *d_stream, uint64_t len, const uint64_t *d_rec_off,

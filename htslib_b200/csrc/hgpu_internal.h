@@ -139,6 +139,12 @@ int hgpu_launch_gzip_inflate(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t 
 int hgpu_launch_crc32(hgpu_ctx *ctx, const uint8_t *d_buf, size_t len, uint32_t *d_partial,
                       uint32_t *h_result, uint32_t crc0, cudaStream_t st);
 
+// hgpu_bam_index_records_dev over a window of a longer record stream (bam_unpack.cu): a record that runs past len ends the
+// walk instead of breaking the chain, and *d_tail (device) receives where the walk stopped (len when whole records fill it)
+int hgpu_bam_records_window_dev(hgpu_ctx *ctx, const uint8_t *d_stream, uint64_t len, const uint64_t *d_hint_off,
+                                uint64_t n_hint, uint64_t *d_rec_off, uint64_t rec_cap, uint64_t *d_n_rec, uint64_t *d_tail,
+                                cudaStream_t st);
+
 int hgpu_launch_crc32_batch(hgpu_ctx *ctx, const uint8_t *d_buf, const uint64_t *d_off, const uint32_t *d_len, uint32_t n,
                             uint32_t *d_crc, cudaStream_t st);
 

@@ -448,6 +448,31 @@ int hgpu_bam_layout_dev(hgpu_ctx *ctx, const uint8_t *d_stream, uint64_t len,
                         const uint64_t *d_rec_off, uint64_t n,
                         uint64_t *d_data_off, uint64_t *d_seq_off, void *stream);
 
+/* BAI / CSI index of a whole BAM image in host memory — sam_index_build3(fn, fnidx, min_shift, 0) (sam.c:994-1074).
+ * *out (malloc'd, *out_len bytes) is the index file exactly as the reference writes it:
+ *   min_shift <= 0: BAI (min_shift 14, 5 levels), uncompressed;
+ *   min_shift > 0:  CSI with hts_adjust_csi_settings (hts.c:2372) applied to the longest @SQ length, BGZF-compressed on the
+ *                   device at the default level in 0xff00-byte payloads plus the EOF block (the compressed bytes are this
+ *                   library's; they inflate to the reference's file).
+ * The image is inflated and walked on the device in windows of whole BGZF blocks of at most window_bytes uncompressed bytes
+ * (at least one block; a record left open at a window's end is carried into the next); 0 picks the size from free
+ * device memory.  Per-record data stays on the device.  Returns HGPU_OK, or:
+ *   HGPU_IDX_ERR_PUSH  hts_idx_push refuses record *bad (unsorted positions, a reference that returns, a placed record after
+ *                      unplaced ones, a position past the format's range — BAI holds 2^29);
+ *   HGPU_IDX_ERR_READ  sam_read1 fails (< -1) on record *bad (broken or truncated chain, bam_read1's -4 cases including the
+ *                      CIGAR/query-length check after the CG-tag rewrite and corrupt aux data before the CG tag, tid or mtid
+ *                      outside the header); *bad = -1 when bam_hdr_read refuses the header;
+ *   HGPU_BGZF_ERR_*    a block fails (bad header, inflate error, CRC, inflated size != ISIZE), *bad = its index; a block is
+ *                      reported as soon as its window inflates, before the records of that window are looked at;
+ *   HGPU_ERR_ARG       not BGZF, or not BAM (a BGZF-compressed SAM needs the text parser, which stays on the host). */
+#define HGPU_IDX_ERR_READ  (-10)
+#define HGPU_IDX_ERR_PUSH  (-11)
+int hgpu_bam_index_build_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, int min_shift,
+                              uint64_t window_bytes, uint8_t **out, uint64_t *out_len, int64_t *bad);
+/* milliseconds of the last hgpu_bam_index_build_host: ms2[0] device time of the windows (CUDA events from the moment a
+ * window's compressed bytes are in HBM to the end of its index kernels, summed), ms2[1] host finishing (bins, file) */
+void hgpu_bam_index_last_ms(float *ms2);
+
 /* the reference sequences of a file, for the CRAM record decoder and encoder: upper case, @SQ order, back to back */
 typedef struct hgpu_cram_refs { const uint8_t *bases; const uint64_t *off; int32_t n_ref; } hgpu_cram_refs;
 

@@ -520,6 +520,74 @@ def cram_decode_records(ctx, file_np, blocks, udata, udata_off, fasta=None, pref
     return _records_out(out, free)
 
 
+# CRAM_OPT_REQUIRED_FIELDS bits (htslib's SAM_*, hts.h:279-291; HGPU_SAM_* in htsgpu.h)
+SAM_QNAME, SAM_FLAG, SAM_RNAME, SAM_POS, SAM_MAPQ, SAM_CIGAR, SAM_RNEXT = 0x1, 0x2, 0x4, 0x8, 0x10, 0x20, 0x40
+SAM_PNEXT, SAM_TLEN, SAM_SEQ, SAM_QUAL, SAM_AUX, SAM_RGAUX, SAM_ALL = 0x80, 0x100, 0x200, 0x400, 0x800, 0x1000, 0x7fffffff
+
+
+def _cram_refs(fasta):
+    """(CramRefs pointer or None, arrays to keep alive) for load_fasta_upper's (bases, offsets)."""
+    import numpy as np
+    if fasta is None:
+        return None, None
+    keep = (np.ascontiguousarray(fasta[0]), np.ascontiguousarray(fasta[1]))
+    refs = CramRefs()
+    refs.bases = keep[0].ctypes.data; refs.off = keep[1].ctypes.data; refs.n_ref = len(keep[1]) - 1
+    return C.byref(refs), (keep, refs)
+
+
+def cram_required_blocks(blocks, udata, udata_off, required_fields, _entry=None):
+    """hgpu_cram_required_blocks: uint8 array, 1 for every block a decode of `required_fields` reads.  Only the header
+    blocks (content types 0 / 1 / 2) of udata need to be uncompressed.  _entry: (function, error) of another build."""
+    import numpy as np
+    used = np.zeros(len(blocks) + 1, dtype=np.uint8)
+    barr = np.ascontiguousarray(blocks)
+    if _entry is None:
+        L = lib()
+        fn, err = L.hgpu_cram_required_blocks, last_error
+    else:
+        fn, err = _entry
+    fn.restype = C.c_long
+    fn.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
+    n = fn(barr.ctypes.data, len(blocks), udata.ctypes.data, udata_off.ctypes.data, required_fields, used.ctypes.data)
+    if n < 0:
+        raise HgpuError("cram_required_blocks: %s" % err())
+    return used[:len(blocks)]
+
+
+def cram_decode_records_fields(ctx, file_np, blocks, udata, udata_off, fasta=None, prefix=b"", decode_md=0, required_fields=0, _entry=None):
+    """cram_decode_records for a field subset (hgpu_cram_decode_records_fields_host): what sam_read1 returns after
+    hts_set_opt(CRAM_OPT_REQUIRED_FIELDS, required_fields).  Blocks cram_required_blocks marks unused may hold anything.
+    _entry: (function, free, error) of another build of the same entry point (tests/hostsim)."""
+    refs, keep = _cram_refs(fasta)
+    out = CramRecords()
+    if _entry is None:
+        L = lib()
+        fn, free, err = L.hgpu_cram_decode_records_fields_host, L.hgpu_cram_records_free, last_error
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p, C.c_int,
+                       C.c_uint32, C.c_void_p]
+        rc = fn(ctx.h, file_np.ctypes.data, file_np.size, blocks.ctypes.data, len(blocks), udata.ctypes.data, udata_off.ctypes.data, refs,
+                prefix, decode_md, required_fields, C.byref(out))
+    else:
+        fn, free, err = _entry
+        rc = fn(file_np.ctypes.data, file_np.size, blocks.ctypes.data, len(blocks), udata.ctypes.data, udata_off.ctypes.data, refs,
+                prefix, decode_md, required_fields, C.byref(out))
+    if rc != 0:
+        raise HgpuError("cram_decode_records_fields: %d %s" % (rc, err()))
+    return _records_out(out, free)
+
+
+def cram_decode_file_fields(ctx, file_np, fasta=None, prefix=b"", decode_md=0, required_fields=0):
+    """hgpu_cram_decode_file_fields_host: scan, uncompress only the blocks the fields need, decode those fields."""
+    L = lib()
+    refs, keep = _cram_refs(fasta)
+    out = CramRecords()
+    L.hgpu_cram_decode_file_fields_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_int, C.c_uint32, C.c_void_p]
+    rc = L.hgpu_cram_decode_file_fields_host(ctx.h, file_np.ctypes.data, file_np.size, refs, prefix, decode_md, required_fields, C.byref(out))
+    if rc != 0:
+        raise HgpuError("cram_decode_file_fields: %d %s" % (rc, last_error()))
+    return _records_out(out, L.hgpu_cram_records_free)
+
 
 def bgzf_scan(file_np):
     """BSIZE-chain walk: returns (off u64[n], len u32[n], isize u32[n]) or raises on a bad block."""

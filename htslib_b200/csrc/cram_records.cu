@@ -64,6 +64,19 @@ struct HRd {
     }
 };
 
+// cram_dependent_data_series walks the series in this order (cram/cram_decode.c:559-564); bit i of a slice's data-series
+// mask stands for series i here.  Index 27 (QQ) is therefore tested and set as 1 << 27, which is CRAM_BB_len, not CRAM_QQ:
+// the reference's quirk, kept, so that exactly its blocks are selected.
+const int k_i_to_id[28] = {DS_BF, DS_AP, DS_FP, DS_RL, DS_DL, DS_NF, DS_BA, DS_QS, DS_FC, DS_FN, DS_BS, DS_IN, DS_RG, DS_MQ,
+                           DS_TL, DS_RN, DS_NS, DS_NP, DS_TS, DS_MF, DS_CF, DS_RI, DS_RS, DS_PD, DS_HC, DS_SC, DS_BB, DS_QQ};
+
+struct BlockIds { int32_t id[2]; };              // cram_codec_to_id of one codec: -2 no block, -1 CORE, else a content id
+
+struct SeriesBlocks {                            // per table: the blocks every series and tag codec reads
+    BlockIds series[28]; uint8_t present[28];
+    std::vector<BlockIds> tags;                  // every tag codec, a key defined twice included (the reference walks them all)
+};
+
 struct Build {                                   // pools shared by all tables of one call
     std::vector<Table> tables;
     std::vector<Codec> cpool;
@@ -73,6 +86,7 @@ struct Build {                                   // pools shared by all tables o
     std::vector<std::map<int32_t, int32_t>> ext_of;      // per table: content id -> dense index
     std::vector<uint32_t> tl_max;                        // per table: longest tag line
     std::vector<uint8_t> usable;                         // per table: 0 = an encoding the device table does not model
+    std::vector<SeriesBlocks> blocks_of;                 // per table
 };
 
 int32_t dense_ext(std::map<int32_t, int32_t> &m, int32_t id)
@@ -189,10 +203,35 @@ const SeriesKey k_series[] = {
     {"DL", DS_DL, T_INT}, {"BA", DS_BA, T_BYTE}, {"BB", DS_BB, T_BYTE_ARRAY}, {"RS", DS_RS, T_INT}, {"PD", DS_PD, T_INT}, {"HC", DS_HC, T_INT},
     {"MQ", DS_MQ, T_INT}, {"RN", DS_RN, T_BYTE_ARRAY_BLOCK}, {"QS", DS_QS, T_BYTE}, {"QQ", DS_QQ, T_BYTE_ARRAY}, {"TL", DS_TL, T_INT}};
 
+// cram_codec_to_id (cram/cram_codecs.c:3968-4016); content_id: dense external index -> content id
+int32_t codec_block(const Build &B, const std::vector<int32_t> &content_id, const Codec &c, int32_t *id2)
+{
+    int32_t b1 = -2, b2 = -2;
+    switch (c.kind) {
+    case K_HUFFMAN: b1 = c.ncodes == 1 ? -2 : -1; break;
+    case K_BETA: case K_SUBEXP: case K_GAMMA: b1 = -1; break;
+    case K_EXTERNAL: case K_BYTE_ARRAY_STOP: b1 = content_id[(size_t)c.a]; break;
+    case K_BYTE_ARRAY_LEN:
+        b1 = codec_block(B, content_id, B.cpool[(size_t)c.a], nullptr);
+        b2 = codec_block(B, content_id, B.cpool[(size_t)c.b], nullptr);
+        break;
+    default: break;
+    }
+    if (id2) *id2 = b2;
+    return b1;
+}
+BlockIds codec_blocks(const Build &B, const std::vector<int32_t> &content_id, const Codec &c)
+{
+    BlockIds r;
+    r.id[0] = codec_block(B, content_id, c, &r.id[1]);
+    return r;
+}
+
 // cram_decode_compression_header :144-538.  0 ok (B.usable says whether the device can take it), -1 malformed.
 int build_table(Build &B, const uint8_t *hdr, uint32_t len)
 {
     Table T;
+    std::vector<Codec> tc_all;
     memset(&T, 0, sizeof T);
     std::map<int32_t, int32_t> ext;
     uint8_t usable = 1;
@@ -273,7 +312,7 @@ int build_table(Build &B, const uint8_t *hdr, uint32_t len)
         const int32_t cnt = r.itf8();
         if (r.err || msz < 0 || cnt < 0) return -1;
         T.tag_off = (uint32_t)B.tagkeys.size();
-        std::vector<Codec> tc;
+        std::vector<Codec> tc, tc_seen;
         for (int32_t i = 0; i < cnt; i++) {
             if (r.e - r.p < 6) return -1;
             const uint32_t key = (uint32_t)r.itf8();
@@ -284,22 +323,106 @@ int build_table(Build &B, const uint8_t *hdr, uint32_t len)
             if (rc < 0) return -1;
             if (rc > 0) usable = 0;
             r.p += sz;
+            tc_seen.push_back(c);
             // map_find walks a list the parser prepended to: the LAST definition of a key is found first
             bool dup = false;
             for (size_t k = 0; k < tc.size(); k++) if (B.tagkeys[T.tag_off + k] == key) { tc[k] = c; dup = true; }
             if (!dup) { B.tagkeys.push_back(key); tc.push_back(c); }
         }
         if (r.err || r.p - start != msz) return -1;
+        tc_all.swap(tc_seen);
         T.n_tags = (uint32_t)tc.size();
         T.tag_codec_off = (uint32_t)B.cpool.size();
         B.cpool.insert(B.cpool.end(), tc.begin(), tc.end());
     }
     T.n_ext = (uint32_t)ext.size();
+    {
+        std::vector<int32_t> content_id(ext.size());
+        for (const auto &kv : ext) content_id[(size_t)kv.second] = kv.first;
+        SeriesBlocks Q;
+        for (int i = 0; i < 28; i++) {
+            const Codec &c = T.ds[k_i_to_id[i]];
+            Q.present[i] = c.kind != K_NONE;
+            Q.series[i] = codec_blocks(B, content_id, c);
+        }
+        for (const Codec &c : tc_all) Q.tags.push_back(codec_blocks(B, content_id, c));
+        B.blocks_of.push_back(Q);
+    }
     B.tables.push_back(T);
     B.ext_of.push_back(ext);
     B.tl_max.push_back(tl_max);
     B.usable.push_back(usable);
     return 0;
+}
+
+bool subset_mode(int32_t req) { return req != 0 && req != SAM_ALL; }
+
+// cram_dependent_data_series (cram/cram_decode.c:553-869) for one slice of table `table`: returns the slice's data-series
+// mask and sets used[k] for its blocks sb[0 .. nb) (sb[0] is the CORE block, uncompressed whatever the mask, :618-620).  The
+// embedded reference block is used too (:2412-2426).  Outside subset mode every block is used and every series read.
+uint32_t select_series(const Build &B, int32_t table, int32_t req, const hgpu_cram_block *sb, int32_t nb, int32_t ref_id,
+                       int32_t ref_base_id, uint8_t *used)
+{
+    if (!subset_mode(req)) { memset(used, 1, (size_t)nb); return CRAM_ALL; }
+    const Table &T = B.tables[(size_t)table];
+    const SeriesBlocks &Q = B.blocks_of[(size_t)table];
+    uint32_t ds = 0;                                                        // :574-616
+    if (req & SAM_QNAME) ds |= CRAM_RN;
+    if (req & SAM_FLAG) ds |= CRAM_BF;
+    if (req & SAM_RNAME) ds |= CRAM_RI | CRAM_BF;
+    if (req & SAM_POS) ds |= CRAM_AP | CRAM_BF;
+    if (req & SAM_MAPQ) ds |= CRAM_MQ;
+    if (req & SAM_CIGAR) ds |= CRAM_CIGAR;
+    if (req & SAM_RNEXT) ds |= CRAM_CF | CRAM_NF | CRAM_RI | CRAM_NS | CRAM_BF;
+    if (req & SAM_PNEXT) ds |= CRAM_CF | CRAM_NF | CRAM_AP | CRAM_NP | CRAM_BF;
+    if (req & SAM_TLEN) ds |= CRAM_CF | CRAM_NF | CRAM_AP | CRAM_TS | CRAM_BF | CRAM_MF | CRAM_RI | CRAM_CIGAR;
+    if (req & SAM_SEQ) ds |= CRAM_SEQ;
+    if (req & SAM_QUAL) ds |= CRAM_QUAL;
+    if (req & SAM_AUX) ds |= CRAM_RG | CRAM_TL | CRAM_aux;
+    if (req & SAM_RGAUX) ds |= CRAM_RG | CRAM_BF;
+
+    memset(used, 0, (size_t)nb);
+    bool core_used = false;
+    auto mark = [&](int32_t id) {
+        if (id == -1) core_used = true;
+        else if (id >= 0) for (int32_t k = 0; k < nb; k++) if (sb[k].content_type == 4 && sb[k].content_id == id) used[k] = 1;
+    };
+    auto reads_used = [&](int32_t id) {
+        if (id == -1) return core_used;
+        for (int32_t k = 0; id >= 0 && k < nb; k++) if (sb[k].content_type == 4 && sb[k].content_id == id && used[k]) return true;
+        return false;
+    };
+    // both blocks of a codec, as the reference's `for (;;)` over bnum1 / bnum2 visits them
+    auto each = [](const BlockIds &b, auto &&f) { f(b.id[0]); if (b.id[1] != -2 && b.id[1] != b.id[0]) f(b.id[1]); };
+    uint32_t orig;
+    do {
+        const uint32_t feat = CRAM_RS | CRAM_PD | CRAM_HC | CRAM_QS | CRAM_IN | CRAM_SC | CRAM_BS | CRAM_DL | CRAM_BA | CRAM_BB | CRAM_QQ;
+        if (ds & feat) ds |= CRAM_FC | CRAM_FP;                            // :645-678
+        if (ds & (CRAM_SEQ | CRAM_CIGAR)) ds |= CRAM_RL;
+        if (ds & CRAM_FP) ds |= CRAM_FC;
+        if (ds & CRAM_FC) ds |= CRAM_FN;
+        if (ds & CRAM_aux) ds |= CRAM_TL;
+        if (ds & CRAM_MF) ds |= CRAM_CF;
+        if (ds & CRAM_MQ) ds |= CRAM_BF;
+        if (ds & CRAM_BS) ds |= CRAM_RI;
+        if (ds & (CRAM_MF | CRAM_NS | CRAM_NP | CRAM_TS | CRAM_NF)) ds |= CRAM_CF;
+        if (!T.read_names_included && (ds & CRAM_RN)) ds |= CRAM_CF | CRAM_NF;
+        if (ds & (CRAM_BA | CRAM_QS | CRAM_BB | CRAM_QQ)) ds |= CRAM_BF | CRAM_CF | CRAM_RL;
+        if (ds & CRAM_FN) ds |= CRAM_SC | CRAM_IN | CRAM_BB;
+        orig = ds;
+        for (int i = 0; i < 28; i++)                                        // the blocks the series read (:683-723)
+            if (((ds >> i) & 1) && Q.present[i]) each(Q.series[i], mark);
+        if ((req & SAM_AUX) || (ds & CRAM_aux))                             // :726-773
+            for (const BlockIds &b : Q.tags) each(b, mark);
+        for (int i = 0; i < 28; i++)                                        // series sharing a used block join (:777-816)
+            if (Q.present[i]) each(Q.series[i], [&](int32_t id) { if (reads_used(id)) ds |= 1u << i; });
+        for (const BlockIds &b : Q.tags)                                    // :819-864: a tag on CORE always pulls the tags in
+            each(b, [&](int32_t id) { if (id == -1 || reads_used(id)) ds |= CRAM_aux; });
+    } while (orig != ds);
+    if (nb > 0) used[0] = 1;
+    if (ref_id >= 0 && ref_base_id >= 0)
+        for (int32_t k = 0; k < nb; k++) if (sb[k].content_type == 4 && sb[k].content_id == ref_base_id) { used[k] = 1; break; }
+    return ds;
 }
 
 struct HeaderInfo { std::vector<int64_t> sq_len; std::vector<std::string> rg; int32_t unknown_rg = -1; };
@@ -447,7 +570,7 @@ CRAMREC_HD void slice_body(const Args &A, uint32_t si, uint32_t lane, uint32_t n
             D.ref = A.P.udata + e.off;
             D.ref_start = S.ref_seq_start;
             D.ref_end = (int64_t)S.ref_seq_start + S.ref_seq_span - 1;
-        } else if (!D.T->no_ref) {
+        } else if (!D.T->no_ref && (S.req & SAM_SEQ)) {                  // without SEQ the reference is not fetched (:2439)
             if (!A.R.bases || S.ref_seq_id >= A.R.n_ref) rc = ERR_NOREF;
             else {
                 const int64_t flen = (int64_t)(A.R.off[S.ref_seq_id + 1] - A.R.off[S.ref_seq_id]);
@@ -459,9 +582,10 @@ CRAMREC_HD void slice_body(const Args &A, uint32_t si, uint32_t lane, uint32_t n
         }
     }
     Rec *recs = A.recs + S.rec0;
-    if (rc == ERR_NONE) rc = D.decode_slice(S, recs, A.nrg, A.unknown_rg);
+    if (rc == ERR_NONE) rc = S.req == SAM_ALL ? D.template decode_slice<false>(S, recs, A.nrg, A.unknown_rg)
+                                              : D.template decode_slice<true>(S, recs, A.nrg, A.unknown_rg);
     W::sync();
-    if (rc == ERR_NONE && slice_xref(recs, S.n_records)) rc = ERR_DECODE;      // every lane runs it on the same data, same stores
+    if (rc == ERR_NONE && slice_xref(recs, S.n_records, S.req)) rc = ERR_DECODE;      // every lane runs it on the same data, same stores
     W::sync();
     // sizes: lanes take records
     uint64_t run = 0;
@@ -469,7 +593,7 @@ CRAMREC_HD void slice_body(const Args &A, uint32_t si, uint32_t lane, uint32_t n
         const int32_t r = base + (int32_t)lane;
         int64_t sz = 0;
         if (r < S.n_records && rc == ERR_NONE) {
-            sz = bam_size(recs, S.n_records, r, A.prefix_len, S.record_counter, A.rg_len, A.nrg);
+            sz = bam_size(recs, S.n_records, r, A.prefix_len, S.record_counter, A.rg_len, A.nrg, S.req);
             if (sz < 0) sz = 0;                                               // cram_to_bam fails on this record: flagged by the fill pass
         }
         uint64_t inc = (uint64_t)sz;
@@ -499,10 +623,10 @@ CRAMREC_HD void fill_body(const Args &A, uint64_t g)
     if (st == ERR_NONE) {
         const Rec *recs = A.recs + S.rec0;
         const int32_t r = (int32_t)(g - S.rec0);
-        if (bam_size(recs, S.n_records, r, A.prefix_len, S.record_counter, A.rg_len, A.nrg) < 0) st = ERR_DECODE;
+        if (bam_size(recs, S.n_records, r, A.prefix_len, S.record_counter, A.rg_len, A.nrg, S.req) < 0) st = ERR_DECODE;
         else if (bam_fill<W>(recs, S.n_records, r, A.prefix, A.prefix_len, S.record_counter, A.scratch + S.name_off, A.scratch + S.seq_off,
                              A.scratch + S.seq_off + S.seq_cap, A.scratch + S.aux_off, reinterpret_cast<const uint32_t *>(A.scratch + S.cig_off),
-                             A.rg_names, A.rg_off, A.rg_len, core, A.data + off)) st = ERR_DECODE;
+                             A.rg_names, A.rg_off, A.rg_len, S.req, core, A.data + off)) st = ERR_DECODE;
     }
     A.core[g] = core;
     A.rec_status[g] = st;
@@ -523,9 +647,11 @@ __global__ void __launch_bounds__(128) cram_bam_fill_kernel(Args A)
 
 int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n_blocks,
                 const uint8_t *udata, const uint64_t *udata_off, const hgpu_cram_refs *refs, const char *name_prefix, int decode_md,
-                hgpu_cram_records *out, hgpu_cram_records_dev *dev = nullptr)
+                int32_t req, hgpu_cram_records *out, hgpu_cram_records_dev *dev = nullptr)
 {
     if (dev) memset(dev, 0, sizeof *dev);
+    if (subset_mode(req) && !(req & SAM_AUX)) decode_md = 0;            // cram_decode.c:605-607
+    // req == 0 reads every series like SAM_ALL, but cram_decode_slice_xref and cram_to_bam test the mask itself
     if (!file || !blocks || !udata || !udata_off || !out) { hgpu_set_error("cram records: null argument"); return HGPU_ERR_ARG; }
     memset(out, 0, sizeof *out);
     if (file_len < 26 || memcmp(file, "CRAM", 4) != 0 || file[4] != 3) { hgpu_set_error("cram records: CRAM 3.x only"); return HGPU_ERR_ARG; }
@@ -547,6 +673,7 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
     uint64_t udata_end = 0;
     for (uint32_t i = 0; i < n_blocks; i++) udata_end = std::max<uint64_t>(udata_end, udata_off[i] + blocks[i].uncomp_size);
     const uint32_t prefix_len = name_prefix ? (uint32_t)strlen(name_prefix) : 0;
+    std::vector<uint8_t> used;
 
     for (uint32_t i = 0; i < n_blocks; i++) {
         const hgpu_cram_block &b = blocks[i];
@@ -578,6 +705,11 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
             S.ref_base_ext = -1;
             S.ext_off = (uint32_t)ext.size();
             ext.resize(ext.size() + T.n_ext + 1, Ext{0, 0xffffffffu, 0});
+            const hgpu_cram_container &C = conts[b.container < (uint32_t)nc ? b.container : 0];
+            used.resize((size_t)sh.n_blocks);
+            S.ds = select_series(B, cur_table, req, blocks + i + 1, sh.n_blocks, sh.ref_id, sh.ref_base_id, used.data());
+            S.req = req;
+            S.cont_ref_start = C.start;
             bool have_core = false;
             uint64_t blk_bytes = 0;
             for (int32_t k = 1; k <= sh.n_blocks; k++) {
@@ -599,14 +731,14 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
             bool ok = B.usable[(size_t)cur_table] && have_core && blocks[i + 1].content_type == 5;
             if (sh.ref_base_id >= 0 && sh.ref_id >= 0 && S.ref_base_ext < 0) ok = false;
             // arenas
-            const hgpu_cram_container &C = conts[b.container < (uint32_t)nc ? b.container : 0];
             const uint64_t nr = (uint64_t)S.n_records;
             // total read length of the slice: exact where RL is a byte stream of ITF8 values or a constant (what the writers
-            // emit); the container header's base count otherwise (htslib itself miscounts it for multi-reference containers)
+            // emit); the container header's base count otherwise (htslib itself miscounts it for multi-reference containers),
+            // and when RL is not read (its block may not be uncompressed then)
             uint64_t bases = C.bases > 0 ? 2 * (uint64_t)C.bases + blk_bytes : blk_bytes;
             {
                 const Codec &rl = T.ds[DS_RL];
-                if (rl.kind == K_EXTERNAL && ext[S.ext_off + (uint32_t)rl.a].size != 0xffffffffu) {
+                if (rl.kind == K_EXTERNAL && (S.ds & CRAM_RL) && ext[S.ext_off + (uint32_t)rl.a].size != 0xffffffffu) {
                     const Ext &e = ext[S.ext_off + (uint32_t)rl.a];
                     HRd rr{udata + e.off, udata + e.off + e.size};
                     uint64_t sum = 0;
@@ -797,6 +929,37 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
     return HGPU_OK;
 }
 
+// hgpu_cram_required_blocks: the slice walk of decode_impl, header blocks only, with select_series per slice
+long required_blocks(const hgpu_cram_block *blocks, uint32_t n_blocks, const uint8_t *udata, const uint64_t *udata_off, int32_t req, uint8_t *used)
+{
+    if (!blocks || !udata || !udata_off || !used) { hgpu_set_error("cram required blocks: null argument"); return -1; }
+    const bool subset = subset_mode(req);
+    for (uint32_t i = 0; i < n_blocks; i++) used[i] = !subset || blocks[i].content_type <= 2;
+    if (!subset) return (long)n_blocks;
+    Build B;
+    int32_t cur_table = -1;
+    std::vector<int32_t> ids(10000);
+    for (uint32_t i = 0; i < n_blocks; i++) {
+        const hgpu_cram_block &b = blocks[i];
+        const uint8_t *pay = udata + udata_off[i];
+        if (b.content_type == 1) {
+            if (build_table(B, pay, b.uncomp_size)) { hgpu_set_error("cram required blocks: malformed compression header (block %u)", i); return -1; }
+            cur_table = (int32_t)B.tables.size() - 1;
+        } else if (b.content_type == 2) {
+            hgpu_cram_slice sh;
+            if (cur_table < 0 || hgpu_cram_parse_slice_header(pay, b.uncomp_size, 3, &sh, ids.data(), (long)ids.size()) < 0 ||
+                sh.n_blocks < 1 || (uint64_t)i + (uint64_t)sh.n_blocks >= (uint64_t)n_blocks + 1) {
+                hgpu_set_error("cram required blocks: malformed slice header (block %u)", i); return -1;
+            }
+            select_series(B, cur_table, req, blocks + i + 1, sh.n_blocks, sh.ref_id, sh.ref_base_id, used + i + 1);
+            i += (uint32_t)sh.n_blocks;
+        }
+    }
+    long n = 0;
+    for (uint32_t i = 0; i < n_blocks; i++) n += used[i];
+    return n;
+}
+
 }  // namespace
 
 extern "C" void hgpu_cram_records_free(hgpu_cram_records *r)
@@ -810,13 +973,28 @@ extern "C" void hgpu_cram_records_free(hgpu_cram_records *r)
 extern "C" int hostsim_cram_decode_records(const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n_blocks,
         const uint8_t *udata, const uint64_t *udata_off, const hgpu_cram_refs *refs, const char *name_prefix, int decode_md, hgpu_cram_records *out)
 {
-    try { return decode_impl(nullptr, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md, out); }
+    try { return decode_impl(nullptr, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md, SAM_ALL, out); }
     catch (...) { hgpu_set_error("internal error"); return HGPU_ERR_NOMEM; }
 }
+extern "C" int hostsim_cram_decode_records_fields(const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n_blocks,
+        const uint8_t *udata, const uint64_t *udata_off, const hgpu_cram_refs *refs, const char *name_prefix, int decode_md,
+        uint32_t required_fields, hgpu_cram_records *out)
+{
+    try { return decode_impl(nullptr, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md, (int32_t)required_fields, out); }
+    catch (...) { hgpu_set_error("internal error"); return HGPU_ERR_NOMEM; }
+}
+extern "C" long hostsim_cram_required_blocks(const hgpu_cram_block *blocks, uint32_t n_blocks, const uint8_t *udata, const uint64_t *udata_off,
+        uint32_t required_fields, uint8_t *used)
+{
+    try { return required_blocks(blocks, n_blocks, udata, udata_off, (int32_t)required_fields, used); }
+    catch (...) { hgpu_set_error("internal error"); return -1; }
+}
 #else
-// scan + cram_uncompress_block for every block + record decode: a CRAM file image in, bam1_t records out
+// scan + cram_uncompress_block + record decode: a CRAM file image in, bam1_t records out.  With a field subset the header
+// blocks are uncompressed first, then only the blocks the selection uses: the others are neither uncompressed nor
+// CRC-checked, as in the reference (the CRC check lives in cram_uncompress_block, cram_io.c:1585)
 static int decode_file_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_refs *refs, const char *name_prefix,
-                            int decode_md, hgpu_cram_records *out)
+                            int decode_md, int32_t req, hgpu_cram_records *out)
 {
     if (!out) { hgpu_set_error("cram file: null argument"); return HGPU_ERR_ARG; }
     memset(out, 0, sizeof *out);
@@ -828,13 +1006,44 @@ static int decode_file_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_le
     std::vector<uint64_t> off((size_t)nb + 1, 0);
     for (long i = 0; i < nb; i++) off[(size_t)i + 1] = off[(size_t)i] + (((uint64_t)blocks[(size_t)i].uncomp_size + 15) & ~15ull);
     std::vector<uint8_t> udata(off[(size_t)nb] + 16);
-    std::vector<uint32_t> got((size_t)nb + 1);
-    std::vector<int32_t> st((size_t)nb + 1);
-    int rc = hgpu_cram_uncompress_blocks_host(ctx, file, file_len, blocks.data(), (uint32_t)nb, udata.data(), off.data(), got.data(), st.data());
-    if (rc) return rc;
-    for (long i = 0; i < nb; i++)
-        if (st[(size_t)i] != HGPU_OK) { hgpu_set_error("cram file: block %ld (method %d) did not uncompress: status %d", i, blocks[(size_t)i].method, st[(size_t)i]); return st[(size_t)i]; }
-    return decode_impl(ctx, file, file_len, blocks.data(), (uint32_t)nb, udata.data(), off.data(), refs, name_prefix, decode_md, out);
+    // uncompress the blocks idx[0 .. n) (all of them when idx is null), block i to dst + dst_off[i].  The call writes back the
+    // whole span between its first and last slot, so blocks uncompressed by an earlier call must not lie inside it.
+    auto uncompress = [&](const uint32_t *idx, uint32_t n, uint8_t *dst, const uint64_t *dst_off) -> int {
+        std::vector<hgpu_cram_block> sb;
+        std::vector<uint64_t> so;
+        if (idx) for (uint32_t k = 0; k < n; k++) { sb.push_back(blocks[idx[k]]); so.push_back(dst_off[idx[k]]); }
+        if (n == 0) return HGPU_OK;
+        std::vector<uint32_t> got((size_t)n + 1);
+        std::vector<int32_t> st((size_t)n + 1);
+        int rc = hgpu_cram_uncompress_blocks_host(ctx, file, file_len, idx ? sb.data() : blocks.data(), n, dst, idx ? so.data() : dst_off,
+                                                  got.data(), st.data());
+        if (rc) return rc;
+        for (uint32_t k = 0; k < n; k++) {
+            const uint32_t i = idx ? idx[k] : k;
+            if (st[k] != HGPU_OK) { hgpu_set_error("cram file: block %u (method %d) did not uncompress: status %d", i, blocks[i].method, st[k]); return st[k]; }
+        }
+        return HGPU_OK;
+    };
+    int rc;
+    if (!subset_mode(req)) {
+        if ((rc = uncompress(nullptr, (uint32_t)nb, udata.data(), off.data()))) return rc;
+    } else {
+        // the header blocks into a buffer of their own (packed), the used blocks into the file layout, then the headers joined in
+        std::vector<uint32_t> idx;
+        std::vector<uint64_t> hoff((size_t)nb + 1, 0);
+        uint64_t hbytes = 0;
+        for (uint32_t i = 0; i < (uint32_t)nb; i++)
+            if (blocks[i].content_type <= 2) { idx.push_back(i); hoff[i] = hbytes; hbytes += ((uint64_t)blocks[i].uncomp_size + 15) & ~15ull; }
+        std::vector<uint8_t> hdata(hbytes + 16);
+        if ((rc = uncompress(idx.data(), (uint32_t)idx.size(), hdata.data(), hoff.data()))) return rc;
+        std::vector<uint8_t> used((size_t)nb + 1);
+        if (required_blocks(blocks.data(), (uint32_t)nb, hdata.data(), hoff.data(), req, used.data()) < 0) return HGPU_CRAM_ERR_DECODE;
+        std::vector<uint32_t> body;
+        for (uint32_t i = 0; i < (uint32_t)nb; i++) if (used[i] && blocks[i].content_type > 2) body.push_back(i);
+        if ((rc = uncompress(body.data(), (uint32_t)body.size(), udata.data(), off.data()))) return rc;
+        for (uint32_t i : idx) memcpy(udata.data() + off[i], hdata.data() + hoff[i], blocks[i].uncomp_size);
+    }
+    return decode_impl(ctx, file, file_len, blocks.data(), (uint32_t)nb, udata.data(), off.data(), refs, name_prefix, decode_md, req, out);
 }
 
 extern "C" int hgpu_cram_decode_records_dev(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n_blocks,
@@ -842,7 +1051,7 @@ extern "C" int hgpu_cram_decode_records_dev(hgpu_ctx *ctx, const uint8_t *file, 
         hgpu_cram_records *out, hgpu_cram_records_dev *dev)
 {
     if (!dev) { hgpu_set_error("cram records: null argument"); return HGPU_ERR_ARG; }
-    return hgpu_abi_call([&] { return decode_impl(ctx, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md, out, dev); },
+    return hgpu_abi_call([&] { return decode_impl(ctx, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md, SAM_ALL, out, dev); },
                          HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
 }
 
@@ -855,13 +1064,34 @@ extern "C" void hgpu_cram_records_last_ms(float *slice_decode_ms, float *bam_fil
 extern "C" int hgpu_cram_decode_file_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_refs *refs,
                                           const char *name_prefix, int decode_md, hgpu_cram_records *out)
 {
-    return hgpu_abi_call([&] { return decode_file_impl(ctx, file, file_len, refs, name_prefix, decode_md, out); }, HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
+    return hgpu_abi_call([&] { return decode_file_impl(ctx, file, file_len, refs, name_prefix, decode_md, SAM_ALL, out); }, HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
+}
+
+extern "C" int hgpu_cram_decode_file_fields_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_refs *refs,
+                                                 const char *name_prefix, int decode_md, uint32_t required_fields, hgpu_cram_records *out)
+{
+    return hgpu_abi_call([&] { return decode_file_impl(ctx, file, file_len, refs, name_prefix, decode_md, (int32_t)required_fields, out); },
+                         HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
 }
 
 extern "C" int hgpu_cram_decode_records_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n_blocks,
         const uint8_t *udata, const uint64_t *udata_off, const hgpu_cram_refs *refs, const char *name_prefix, int decode_md, hgpu_cram_records *out)
 {
-    return hgpu_abi_call([&] { return decode_impl(ctx, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md, out); },
+    return hgpu_abi_call([&] { return decode_impl(ctx, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md, SAM_ALL, out); },
                          HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
+}
+
+extern "C" int hgpu_cram_decode_records_fields_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks,
+        uint32_t n_blocks, const uint8_t *udata, const uint64_t *udata_off, const hgpu_cram_refs *refs, const char *name_prefix, int decode_md,
+        uint32_t required_fields, hgpu_cram_records *out)
+{
+    return hgpu_abi_call([&] { return decode_impl(ctx, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md,
+                                                  (int32_t)required_fields, out); }, HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
+}
+
+extern "C" long hgpu_cram_required_blocks(const hgpu_cram_block *blocks, uint32_t n_blocks, const uint8_t *udata, const uint64_t *udata_off,
+                                          uint32_t required_fields, uint8_t *used)
+{
+    return hgpu_abi_call([&] { return required_blocks(blocks, n_blocks, udata, udata_off, (int32_t)required_fields, used); }, -1L, -1L);
 }
 #endif

@@ -33,6 +33,22 @@ namespace cramrec {
 enum DS { DS_BF, DS_CF, DS_RI, DS_RL, DS_AP, DS_RG, DS_RN, DS_MF, DS_NS, DS_NP, DS_TS, DS_NF, DS_TL, DS_FN, DS_FC, DS_FP, DS_DL,
           DS_BA, DS_BS, DS_IN, DS_SC, DS_RS, DS_PD, DS_HC, DS_BB, DS_QQ, DS_MQ, DS_QS, DS_COUNT };
 
+// CRAM_OPT_REQUIRED_FIELDS: the SAM_* bits of htslib/hts.h:279-291, and the data-series bits the reference derives from
+// them (enum cram_fields, cram/cram_structs.h:890-922).  A slice's `ds` selects which series its record loop reads;
+// `req` holds the caller's SAM_* mask for the choices cram_decode_slice / cram_to_bam make on it directly.
+enum : int32_t { SAM_QNAME = 0x1, SAM_FLAG = 0x2, SAM_RNAME = 0x4, SAM_POS = 0x8, SAM_MAPQ = 0x10, SAM_CIGAR = 0x20, SAM_RNEXT = 0x40,
+                 SAM_PNEXT = 0x80, SAM_TLEN = 0x100, SAM_SEQ = 0x200, SAM_QUAL = 0x400, SAM_AUX = 0x800, SAM_RGAUX = 0x1000,
+                 SAM_ALL = 0x7fffffff };
+enum : uint32_t { CRAM_BF = 1u << 0, CRAM_AP = 1u << 1, CRAM_FP = 1u << 2, CRAM_RL = 1u << 3, CRAM_DL = 1u << 4, CRAM_NF = 1u << 5,
+                  CRAM_BA = 1u << 6, CRAM_QS = 1u << 7, CRAM_FC = 1u << 8, CRAM_FN = 1u << 9, CRAM_BS = 1u << 10, CRAM_IN = 1u << 11,
+                  CRAM_RG = 1u << 12, CRAM_MQ = 1u << 13, CRAM_TL = 1u << 14, CRAM_RN = 1u << 15, CRAM_NS = 1u << 16, CRAM_NP = 1u << 17,
+                  CRAM_TS = 1u << 18, CRAM_MF = 1u << 19, CRAM_CF = 1u << 20, CRAM_RI = 1u << 21, CRAM_RS = 1u << 22, CRAM_PD = 1u << 23,
+                  CRAM_HC = 1u << 24, CRAM_SC = 1u << 25, CRAM_BB = 1u << 26, CRAM_BB_len = 1u << 27, CRAM_QQ = 1u << 28,
+                  CRAM_aux = 1u << 30, CRAM_ALL = 0x7fffffffu,
+                  CRAM_CIGAR = CRAM_FN | CRAM_FP | CRAM_FC | CRAM_DL | CRAM_IN | CRAM_SC | CRAM_HC | CRAM_PD | CRAM_RS | CRAM_RL | CRAM_BF,
+                  CRAM_SEQ = CRAM_CIGAR | CRAM_BA | CRAM_BS | CRAM_RL | CRAM_AP | CRAM_BB,
+                  CRAM_QUAL = CRAM_CIGAR | CRAM_RL | CRAM_AP | CRAM_QS | CRAM_QQ };
+
 enum Kind : uint8_t { K_NONE = 0, K_EXTERNAL = 1, K_HUFFMAN = 3, K_BYTE_ARRAY_LEN = 4, K_BYTE_ARRAY_STOP = 5, K_BETA = 6, K_SUBEXP = 7, K_GAMMA = 9 };
 enum Type : uint8_t { T_INT = 1, T_BYTE = 2, T_BYTE_ARRAY = 3, T_BYTE_ARRAY_BLOCK = 4 };   // cram_external_type
 
@@ -63,6 +79,10 @@ struct Slice {
     uint64_t rec0;                   // first record of this slice in the global record arrays
     uint64_t name_off, seq_off, aux_off, cig_off;       // arenas in the scratch buffer (cig_off in bytes, 4-aligned)
     uint32_t name_cap, seq_cap, aux_cap, cig_cap;       // bytes, bytes (seq and qual each), bytes, ops
+    uint32_t ds;                     // data series the record loop reads (CRAM_ALL unless a field subset was asked for)
+    int32_t req;                     // the SAM_* mask (SAM_ALL when none was given)
+    int32_t cont_ref_start;          // the container's ref_seq_start: the position of every record when AP is not read
+    int32_t pad;
 };
 
 struct Rec {                         // cram_record (cram/cram_structs.h:545-590) as far as cram_to_bam reads it
@@ -357,8 +377,12 @@ struct SliceDec {
     CRAMREC_HD int64_t sq_len(int32_t id) const { return R.sq_len[id]; }
 
     // cram_decode_seq :1096-1917.  returns 0 / -1
-    CRAMREC_HD int decode_seq(Rec &cr, int cf, uint8_t *seq, uint8_t *qual, int has_MD, int has_NM)
+    // SUBSET: the record loop of a field subset, gated by the slice's data-series mask; the all-fields instantiation
+    // (SUBSET false, every gate constant) compiles to the loop without gates
+    template <bool SUBSET>
+    CRAMREC_HD int decode_seq(Rec &cr, int cf, uint8_t *seq, uint8_t *qual, int has_MD, int has_NM, uint32_t slice_ds)
     {
+        const uint32_t ds = SUBSET ? slice_ds : CRAM_ALL;
         int32_t prev_pos = 0, fn = 0, i32 = 0;
         int32_t seq_pos = 1;
         uint32_t cig_len = 0, cig_op = CIG_M;
@@ -372,23 +396,30 @@ struct SliceDec {
         const Codec *C = T->ds;
         const int pres_q = cf & CRAM_FLAG_PRESERVE_QUAL_SCORES;
 
-        if (!pres_q) W::fill(qual, 255, (uint32_t)cr.len);
+        if ((ds & CRAM_QS) && !pres_q) W::fill(qual, 255, (uint32_t)cr.len);
         if (cr.cram_flags & CRAM_FLAG_NO_SEQ) decode_md = decode_nm = 0;
         if (decode_md) {
             orig_aux = aux_size;
             if (has_MD == 0) { if (!aux_char('M') || !aux_char('D') || !aux_char('Z')) return -1; }
         }
-        if (C[DS_FN].kind == K_NONE) return -1;
-        if (get_int(C[DS_FN], fn)) return -1;
+        if (ds & CRAM_FN) {
+            if (C[DS_FN].kind == K_NONE) return -1;
+            if (get_int(C[DS_FN], fn)) return -1;
+        }
         ref_pos--;
         cr.cigar = ncigar;
-        if (fn) { if (C[DS_FC].kind == K_NONE || C[DS_FP].kind == K_NONE) return -1; }
+        // without FC and FP the reference skips the features and the implicit match (goto skip_cigar); the selection
+        // makes FP imply FC, so the only partial case is FC alone: the codes are read, nothing else
+        if (fn && (ds & (CRAM_FC | CRAM_FP))) {
+            if (((ds & CRAM_FC) && C[DS_FC].kind == K_NONE) || ((ds & CRAM_FP) && C[DS_FP].kind == K_NONE)) return -1;
+        }
 
-        for (int32_t f = 0; f < fn; f++) {
+        for (int32_t f = 0; f < fn && (ds & (CRAM_FC | CRAM_FP)); f++) {
             int32_t pos = 0;
             uint8_t op = 0;
             if (ncigar + 2 >= cig_cap) { err = ERR_SPACE; return -1; }
-            if (get_byte(C[DS_FC], op)) return -1;
+            if ((ds & CRAM_FC) && get_byte(C[DS_FC], op)) return -1;
+            if (!(ds & CRAM_FP)) continue;
             if (get_int(C[DS_FP], pos)) return -1;
             pos += prev_pos;
             if (pos <= 0) return -1;
@@ -430,11 +461,13 @@ struct SliceDec {
                 seq_pos = pos;
             }
             prev_pos = pos;
+            if (!(ds & CRAM_FC)) break;
 
             switch (op) {
             case 'S': {
                 int32_t out_sz2 = cr.len ? cr.len - (pos - 1) : 1;
                 if (cig_len) { if (!cig_push(cig_len, cig_op)) return -1; cig_len = 0; }
+                if (!(ds & CRAM_SC)) break;
                 if (C[DS_SC].kind != K_NONE) { if (get_array_char(C[DS_SC], cr.len ? &seq[pos - 1] : nullptr, out_sz2)) return -1; }
                 else { if (cr.len) seq[pos - 1] = 'N'; out_sz2 = 1; }
                 if (!cig_push((uint32_t)out_sz2, CIG_S)) return -1;
@@ -444,9 +477,10 @@ struct SliceDec {
             case 'X': {
                 uint8_t base = 0;
                 if (cig_len && cig_op != CIG_M) { if (!cig_push(cig_len, cig_op)) return -1; cig_len = 0; }
-                if (C[DS_BS].kind == K_NONE) return -1;
-                if (get_byte(C[DS_BS], base)) return -1;
-                if (cr.ref_id < 0 || ref_pos >= sq_len(cr.ref_id) || !ref) {
+                if (!(ds & CRAM_BS)) {
+                } else if (C[DS_BS].kind == K_NONE || get_byte(C[DS_BS], base)) {
+                    return -1;
+                } else if (cr.ref_id < 0 || ref_pos >= sq_len(cr.ref_id) || !ref) {
                     if (pos - 1 < cr.len) seq[pos - 1] = T->sub[4][base & 3];
                     if (decode_md || decode_nm) {
                         if (md_dist >= 0 && decode_md) { if (!aux_uint((uint32_t)md_dist)) return -1; }
@@ -463,6 +497,7 @@ struct SliceDec {
                 break; }
             case 'D': {
                 if (cig_len && cig_op != CIG_D) { if (!cig_push(cig_len, cig_op)) return -1; cig_len = 0; }
+                if (!(ds & CRAM_DL)) break;
                 if (C[DS_DL].kind == K_NONE) return -1;
                 if (get_int(C[DS_DL], i32)) return -1;
                 if (i32 < 0) return -1;
@@ -497,6 +532,7 @@ struct SliceDec {
             case 'I': {
                 int32_t out_sz2 = cr.len ? cr.len - (pos - 1) : 1;
                 if (cig_len && cig_op != CIG_I) { if (!cig_push(cig_len, cig_op)) return -1; cig_len = 0; }
+                if (!(ds & CRAM_IN)) break;
                 if (C[DS_IN].kind == K_NONE) return -1;
                 if (get_array_char(C[DS_IN], cr.len ? &seq[pos - 1] : nullptr, out_sz2)) return -1;
                 cig_op = CIG_I;
@@ -504,17 +540,20 @@ struct SliceDec {
                 break; }
             case 'i': {
                 if (cig_len && cig_op != CIG_I) { if (!cig_push(cig_len, cig_op)) return -1; cig_len = 0; }
-                if (C[DS_BA].kind == K_NONE) return -1;
-                { uint8_t b1 = 0; if (get_byte(C[DS_BA], b1)) return -1; if (cr.len) seq[pos - 1] = b1; }
+                if (ds & CRAM_BA) {
+                    if (C[DS_BA].kind == K_NONE) return -1;
+                    uint8_t b1 = 0; if (get_byte(C[DS_BA], b1)) return -1; if (cr.len) seq[pos - 1] = b1;
+                }
                 cig_op = CIG_I;
                 cig_len++; seq_pos++; nm++;
                 break; }
             case 'b': {
                 int32_t len = cr.len ? cr.len - (pos - 1) : 1;
                 if (cig_len && cig_op != CIG_M) { if (!cig_push(cig_len, cig_op)) return -1; cig_len = 0; }
-                if (C[DS_BB].kind == K_NONE) return -1;
-                if (get_array_char(C[DS_BB], cr.len ? &seq[pos - 1] : nullptr, len)) return -1;
-                if (decode_md || decode_nm) {
+                if (!(ds & CRAM_BB)) {
+                } else if (C[DS_BB].kind == K_NONE || get_array_char(C[DS_BB], cr.len ? &seq[pos - 1] : nullptr, len)) {
+                    return -1;
+                } else if (decode_md || decode_nm) {
                     int32_t x;
                     if (md_dist >= 0 && decode_md) { if (!aux_uint((uint32_t)md_dist)) return -1; }
                     for (x = 0; x < len; x++) {
@@ -534,48 +573,57 @@ struct SliceDec {
             case 'q': {
                 int32_t len = cr.len ? cr.len - (pos - 1) : 1;
                 if (cig_len && cig_op != CIG_M) { if (!cig_push(cig_len, cig_op)) return -1; cig_len = 0; }
-                if (C[DS_QQ].kind == K_NONE) return -1;
-                if (!pres_q && cr.len > 0 && qual[0] == 255) W::fill(qual, 30, (uint32_t)cr.len);
-                if (get_array_char(C[DS_QQ], cr.len ? &qual[pos - 1] : nullptr, len)) return -1;
+                if (ds & CRAM_QQ) {
+                    if (C[DS_QQ].kind == K_NONE) return -1;
+                    if ((ds & CRAM_QS) && !pres_q && cr.len > 0 && qual[0] == 255) W::fill(qual, 30, (uint32_t)cr.len);
+                    if (get_array_char(C[DS_QQ], cr.len ? &qual[pos - 1] : nullptr, len)) return -1;
+                }
                 cig_op = CIG_M;
                 break; }
             case 'B': {
                 if (cig_len && cig_op != CIG_M) { if (!cig_push(cig_len, cig_op)) return -1; cig_len = 0; }
-                if (C[DS_BA].kind == K_NONE) return -1;
                 uint8_t b1 = 0, q1 = 0;
-                const int rb = get_byte(C[DS_BA], b1);
-                if (!rb && cr.len) seq[pos - 1] = b1;
-                if (decode_md || decode_nm) {
-                    if (md_dist >= 0 && decode_md) { if (!aux_uint((uint32_t)md_dist)) return -1; }
-                    if (ref_pos >= sq_len(cr.ref_id) || !ref) md_dist = -1;
-                    else {
-                        if (decode_md) {
-                            if (ref_pos >= ref_end) return -1;
-                            if (!aux_char(ref[ref_pos - ref_start + 1])) return -1;
+                int rb = 0, rq = 0;
+                if (ds & CRAM_BA) {
+                    if (C[DS_BA].kind == K_NONE) return -1;
+                    rb = get_byte(C[DS_BA], b1);
+                    if (!rb && cr.len) seq[pos - 1] = b1;
+                    if (decode_md || decode_nm) {
+                        if (md_dist >= 0 && decode_md) { if (!aux_uint((uint32_t)md_dist)) return -1; }
+                        if (ref_pos >= sq_len(cr.ref_id) || !ref) md_dist = -1;
+                        else {
+                            if (decode_md) {
+                                if (ref_pos >= ref_end) return -1;
+                                if (!aux_char(ref[ref_pos - ref_start + 1])) return -1;
+                            }
+                            nm++;
+                            md_dist = 0;
                         }
-                        nm++;
-                        md_dist = 0;
                     }
                 }
-                if (C[DS_QS].kind == K_NONE) return -1;
-                if (!pres_q && cr.len > 0 && qual[0] == 255) W::fill(qual, 30, (uint32_t)cr.len);
-                const int rq = get_byte(C[DS_QS], q1);
-                if (!rq && cr.len) qual[pos - 1] = q1;
+                if (ds & CRAM_QS) {
+                    if (C[DS_QS].kind == K_NONE) return -1;
+                    if (!pres_q && cr.len > 0 && qual[0] == 255) W::fill(qual, 30, (uint32_t)cr.len);
+                    rq = get_byte(C[DS_QS], q1);
+                    if (!rq && cr.len) qual[pos - 1] = q1;
+                }
                 if (rb | rq) return -1;                                    // the reference ORs r and fails the record at the end
                 cig_op = CIG_M;
                 cig_len++; seq_pos++; ref_pos++;
                 break; }
             case 'Q': {
+                if (!(ds & CRAM_QS)) break;
                 if (C[DS_QS].kind == K_NONE) return -1;
                 if (!pres_q && cr.len > 0 && qual[0] == 255) W::fill(qual, 30, (uint32_t)cr.len);
                 { uint8_t q1 = 0; if (get_byte(C[DS_QS], q1)) return -1; if (cr.len) qual[pos - 1] = q1; }
                 break; }
             case 'H': case 'P': case 'N': {
                 const uint32_t cop = op == 'H' ? CIG_H : op == 'P' ? CIG_P : CIG_N;
-                const int ds = op == 'H' ? DS_HC : op == 'P' ? DS_PD : DS_RS;
+                const int series = op == 'H' ? DS_HC : op == 'P' ? DS_PD : DS_RS;
                 if (cig_len && cig_op != cop) { if (!cig_push(cig_len, cig_op)) return -1; cig_len = 0; }
-                if (C[ds].kind == K_NONE) return -1;
-                if (get_int(C[ds], i32)) return -1;
+                if (!(ds & (op == 'H' ? CRAM_HC : op == 'P' ? CRAM_PD : CRAM_RS))) break;
+                if (C[series].kind == K_NONE) return -1;
+                if (get_int(C[series], i32)) return -1;
                 if (i32 < 0) return -1;
                 cig_op = cop;
                 cig_len += i32;
@@ -588,7 +636,7 @@ struct SliceDec {
         }
 
         // implicit match for the bases no feature accounted for
-        if (cr.len >= seq_pos) {
+        if ((ds & CRAM_FC) && (ds & CRAM_FN) && cr.len >= seq_pos) {
             if (ref && cr.ref_id >= 0) {
                 if (ref_pos + cr.len - seq_pos + 1 > sq_len(cr.ref_id)) {
                     const int64_t rlen = sq_len(cr.ref_id) - ref_pos;
@@ -625,15 +673,17 @@ struct SliceDec {
             cig_len += cr.len - seq_pos + 1;
         }
 
-        if (decode_md && md_dist >= 0) { if (!aux_uint((uint32_t)md_dist)) return -1; }
+        if ((ds & CRAM_FN) && decode_md && md_dist >= 0) { if (!aux_uint((uint32_t)md_dist)) return -1; }
         if (cig_len) { if (!cig_push(cig_len, cig_op)) return -1; }
         cr.ncigar = ncigar - cr.cigar;
         cr.aend = ref_pos > cr.apos ? ref_pos : cr.apos;
 
         int r = 0;
-        if (C[DS_MQ].kind == K_NONE) return -1;
-        r |= get_int(C[DS_MQ], cr.mqual);
-        if (pres_q) {
+        if (ds & CRAM_MQ) {
+            if (C[DS_MQ].kind == K_NONE) return -1;
+            r |= get_int(C[DS_MQ], cr.mqual);
+        } else cr.mqual = 40;
+        if ((ds & CRAM_QS) && pres_q) {
             if (C[DS_QS].kind == K_NONE) return -1;
             r |= get_bytes(C[DS_QS], qual, cr.len);
         }
@@ -676,9 +726,12 @@ struct SliceDec {
     }
 
     // cram_decode_aux :2008-2137 (CRAM 3: no '*' placeholders)
-    CRAMREC_HD int decode_aux(Rec &cr, int &has_MD, int &has_NM)
+    template <bool SUBSET>
+    CRAMREC_HD int decode_aux(Rec &cr, int &has_MD, int &has_NM, uint32_t slice_ds)
     {
+        const uint32_t ds = SUBSET ? slice_ds : CRAM_ALL;
         int32_t TL = 0;
+        if (!(ds & (CRAM_TL | CRAM_aux))) { cr.aux = 0; cr.aux_size = 0; return 0; }
         if (T->ds[DS_TL].kind == K_NONE) return -1;
         if (get_int(T->ds[DS_TL], TL) || TL < 0 || (uint32_t)TL >= T->n_tl) return -1;
         const uint8_t *TN = P.td + P.tlidx[T->tl_off + TL];
@@ -686,6 +739,7 @@ struct SliceDec {
         while (TN[ntags * 3] && TN[ntags * 3 + 1] && TN[ntags * 3 + 2]) ntags++;           // strlen / 3
         cr.aux_size = 0;
         cr.aux = aux_size;
+        if (!(ds & CRAM_aux)) return 0;
         for (int i = 0; i < ntags; i++, TN += 3) {
             if (TN[0] == 'M' && TN[1] == 'D') has_MD = (int)(aux_size + 3) * (TN[2] == '*' ? -1 : 1);
             if (TN[0] == 'N' && TN[1] == 'M') has_NM = (int)(aux_size + 3) * (TN[2] == '*' ? -1 : 1);
@@ -712,8 +766,11 @@ struct SliceDec {
     }
 
     // the record loop of cram_decode_slice :2554-2968.  recs: this slice's records.  returns 0 or an ERR_ code
+    template <bool SUBSET>
     CRAMREC_HD int decode_slice(const Slice &S, Rec *recs, int32_t nrg, int32_t unknown_rg)
     {
+        const uint32_t ds = SUBSET ? S.ds : CRAM_ALL;
+        const int32_t req = SUBSET ? S.req : SAM_ALL;
         const Codec *C = T->ds;
         int64_t last_apos = S.ref_seq_start;                                // s->last_apos = s->hdr->ref_seq_start (cram_decode_slice_header)
         int32_t last_ref_id = -9;
@@ -721,18 +778,23 @@ struct SliceDec {
             Rec cr;
             int32_t bf = 0, cf = 0, v = 0;
             int has_MD = 0, has_NM = 0;
-            if (C[DS_BF].kind == K_NONE) return ERR_DECODE;
-            if (get_int(C[DS_BF], bf) || bf < 0 || bf >= 0x1000) return ERR_DECODE;
+            if (ds & CRAM_BF) {
+                if (C[DS_BF].kind == K_NONE) return ERR_DECODE;
+                if (get_int(C[DS_BF], bf) || bf < 0 || bf >= 0x1000) return ERR_DECODE;
+            } else bf = BAM_FUNMAP;
             cr.flags = bf;
-            if (C[DS_CF].kind == K_NONE) return ERR_DECODE;
-            if (get_int(C[DS_CF], cf)) return ERR_DECODE;
+            if (ds & CRAM_CF) {
+                if (C[DS_CF].kind == K_NONE) return ERR_DECODE;
+                if (get_int(C[DS_CF], cf)) return ERR_DECODE;
+            }
             cr.cram_flags = cf;
             cf &= 0xff;                                                     // `unsigned char cf` there
-            if (S.ref_seq_id == -2) {
+            if (S.ref_seq_id == -2 && !(ds & CRAM_RI)) cr.ref_id = -1;
+            else if (S.ref_seq_id == -2) {
                 if (C[DS_RI].kind == K_NONE) return ERR_DECODE;
                 if (get_int(C[DS_RI], cr.ref_id)) return ERR_DECODE;
                 if (cr.ref_id < -1 || cr.ref_id >= R.n_ref) return ERR_DECODE;
-                if (cr.ref_id >= 0 && cr.ref_id != last_ref_id) {
+                if ((req & (SAM_SEQ | SAM_TLEN)) && cr.ref_id >= 0 && cr.ref_id != last_ref_id) {
                     if (!T->no_ref) {
                         if (!R.bases) return ERR_NOREF;
                         ref = R.bases + R.off[cr.ref_id];
@@ -744,24 +806,32 @@ struct SliceDec {
             } else cr.ref_id = S.ref_seq_id;
             if (cr.ref_id < -1 || cr.ref_id >= R.n_ref) return ERR_DECODE;
 
-            if (C[DS_RL].kind == K_NONE) return ERR_DECODE;
-            if (get_int(C[DS_RL], cr.len)) return ERR_DECODE;
-            if (cr.len < 0) return ERR_DECODE;
+            cr.len = 0;
+            if (ds & CRAM_RL) {
+                if (C[DS_RL].kind == K_NONE) return ERR_DECODE;
+                if (get_int(C[DS_RL], cr.len)) return ERR_DECODE;
+                if (cr.len < 0) return ERR_DECODE;
+            }
 
-            if (C[DS_AP].kind == K_NONE) return ERR_DECODE;
-            if (get_int(C[DS_AP], v)) return ERR_DECODE;
-            cr.apos = v;
-            if (T->ap_delta) cr.apos += last_apos;
-            last_apos = cr.apos;
-            if (S.ref_seq_id >= 0 && cr.apos < S.ref_seq_start) return ERR_DECODE;
+            if (ds & CRAM_AP) {
+                if (C[DS_AP].kind == K_NONE) return ERR_DECODE;
+                if (get_int(C[DS_AP], v)) return ERR_DECODE;
+                cr.apos = v;
+                if (T->ap_delta) cr.apos += last_apos;
+                last_apos = cr.apos;
+                if (S.ref_seq_id >= 0 && cr.apos < S.ref_seq_start) return ERR_DECODE;
+            } else cr.apos = S.cont_ref_start;
 
-            if (C[DS_RG].kind == K_NONE) return ERR_DECODE;
-            if (get_int(C[DS_RG], cr.rg)) return ERR_DECODE;
-            if (cr.rg == unknown_rg) cr.rg = -1;
+            cr.rg = -1;
+            if (ds & CRAM_RG) {
+                if (C[DS_RG].kind == K_NONE) return ERR_DECODE;
+                if (get_int(C[DS_RG], cr.rg)) return ERR_DECODE;
+                if (cr.rg == unknown_rg) cr.rg = -1;
+            }
 
             cr.name_len = 0;
             cr.name = name_size;
-            if (T->read_names_included) {
+            if (T->read_names_included && (ds & CRAM_RN)) {
                 int32_t sz = 1;
                 if (C[DS_RN].kind == K_NONE) return ERR_DECODE;
                 if (get_array_block(C[DS_RN], name, name_size, name_cap, sz)) return err ? err : ERR_DECODE;
@@ -770,43 +840,55 @@ struct SliceDec {
 
             cr.mate_pos = 0; cr.mate_line = -1; cr.mate_ref_id = -1; cr.explicit_tlen = CRAMREC_I64_MIN;
             cr.mate_flags = 0; cr.tlen = CRAMREC_I64_MIN;
+            // (cf is 0 when CF is not read, so these branches follow the reference's `(ds & CRAM_CF) && (cf & ...)`)
             if (cf & CRAM_FLAG_DETACHED) {
-                if (C[DS_MF].kind == K_NONE) return ERR_DECODE;
-                if (get_int(C[DS_MF], cr.mate_flags)) return ERR_DECODE;
+                if (ds & CRAM_MF) {
+                    if (C[DS_MF].kind == K_NONE) return ERR_DECODE;
+                    if (get_int(C[DS_MF], cr.mate_flags)) return ERR_DECODE;
+                }
                 if (!T->read_names_included) {
                     int32_t sz = 1;
                     cr.name = name_size;
-                    if (C[DS_RN].kind == K_NONE) return ERR_DECODE;
-                    if (get_array_block(C[DS_RN], name, name_size, name_cap, sz)) return err ? err : ERR_DECODE;
-                    cr.name_len = (uint32_t)sz;
+                    if (ds & CRAM_RN) {
+                        if (C[DS_RN].kind == K_NONE) return ERR_DECODE;
+                        if (get_array_block(C[DS_RN], name, name_size, name_cap, sz)) return err ? err : ERR_DECODE;
+                        cr.name_len = (uint32_t)sz;
+                    }
                 }
-                if (C[DS_NS].kind == K_NONE) return ERR_DECODE;
-                if (get_int(C[DS_NS], cr.mate_ref_id)) return ERR_DECODE;
-                if (cr.mate_ref_id < -1 || cr.mate_ref_id >= R.n_ref) return ERR_DECODE;
-                if (C[DS_NP].kind == K_NONE) return ERR_DECODE;
-                if (get_int(C[DS_NP], v)) return ERR_DECODE;
-                cr.mate_pos = v;
-                if (C[DS_TS].kind == K_NONE) return ERR_DECODE;
-                if (get_int(C[DS_TS], v)) return ERR_DECODE;
-                cr.tlen = v;
+                if (ds & CRAM_NS) {
+                    if (C[DS_NS].kind == K_NONE) return ERR_DECODE;
+                    if (get_int(C[DS_NS], cr.mate_ref_id)) return ERR_DECODE;
+                    if (cr.mate_ref_id < -1 || cr.mate_ref_id >= R.n_ref) return ERR_DECODE;
+                }
+                if (ds & CRAM_NP) {
+                    if (C[DS_NP].kind == K_NONE) return ERR_DECODE;
+                    if (get_int(C[DS_NP], v)) return ERR_DECODE;
+                    cr.mate_pos = v;
+                }
+                if (ds & CRAM_TS) {
+                    if (C[DS_TS].kind == K_NONE) return ERR_DECODE;
+                    if (get_int(C[DS_TS], v)) return ERR_DECODE;
+                    cr.tlen = v;
+                }
             } else if (cf & CRAM_FLAG_MATE_DOWNSTREAM) {
-                if (C[DS_NF].kind == K_NONE) return ERR_DECODE;
-                if (get_int(C[DS_NF], cr.mate_line)) return ERR_DECODE;
-                cr.mate_line += rec + 1;
-                cr.mate_ref_id = -1; cr.tlen = CRAMREC_I64_MIN; cr.mate_pos = 0;
-                if (cf & CRAM_FLAG_EXPLICIT_TLEN) {
+                if (ds & CRAM_NF) {
+                    if (C[DS_NF].kind == K_NONE) return ERR_DECODE;
+                    if (get_int(C[DS_NF], cr.mate_line)) return ERR_DECODE;
+                    cr.mate_line += rec + 1;
+                }
+                if ((cf & CRAM_FLAG_EXPLICIT_TLEN) && (ds & CRAM_TS)) {
                     if (C[DS_TS].kind == K_NONE) return ERR_DECODE;
                     if (get_int(C[DS_TS], v)) return ERR_DECODE;
                     cr.explicit_tlen = v;
                 }
-            } else if (cf & CRAM_FLAG_EXPLICIT_TLEN) {
+            } else if ((cf & CRAM_FLAG_EXPLICIT_TLEN) && (ds & CRAM_TS)) {
                 if (C[DS_TS].kind == K_NONE) return ERR_DECODE;
                 if (get_int(C[DS_TS], v)) return ERR_DECODE;
                 cr.explicit_tlen = v;
             }
 
             cr.aux = aux_size; cr.aux_size = 0;
-            if (decode_aux(cr, has_MD, has_NM)) return err ? err : ERR_DECODE;
+            if (decode_aux<SUBSET>(cr, has_MD, has_NM, ds)) return err ? err : ERR_DECODE;
 
             if ((uint64_t)sq_size + (uint32_t)cr.len > sq_cap) { CRAMREC_TRACE("seq full %u + %d > %u\n", sq_size, cr.len, sq_cap); return ERR_SPACE; }
             cr.seq = cr.qual = sq_size;
@@ -816,20 +898,24 @@ struct SliceDec {
 
             cr.cigar = ncigar; cr.ncigar = 0;
             if (!(bf & BAM_FUNMAP)) {
-                if (cr.apos <= 0) return ERR_DECODE;
-                if (decode_seq(cr, cf, seq, qual, has_MD, has_NM)) return err ? err : ERR_DECODE;
+                if ((ds & CRAM_AP) && cr.apos <= 0) return ERR_DECODE;
+                if (ds & (CRAM_SEQ | CRAM_MQ)) {
+                    if (decode_seq<SUBSET>(cr, cf, seq, qual, has_MD, has_NM, ds)) return err ? err : ERR_DECODE;
+                } else { cr.cigar = 0; cr.ncigar = 0; cr.aend = cr.apos; cr.mqual = 0; }
             } else {
                 cr.cigar = 0; cr.ncigar = 0; cr.aend = cr.apos; cr.mqual = 0;
-                if (cr.len) {
+                if ((ds & CRAM_BA) && cr.len) {
                     if (C[DS_BA].kind == K_NONE) return ERR_DECODE;
                     if (get_bytes(C[DS_BA], seq, cr.len)) return ERR_DECODE;
                 }
                 if (cf & CRAM_FLAG_PRESERVE_QUAL_SCORES) {
-                    if (C[DS_QS].kind == K_NONE) return ERR_DECODE;
-                    if (get_bytes(C[DS_QS], qual, cr.len)) return ERR_DECODE;
+                    if (ds & CRAM_QS) {
+                        if (C[DS_QS].kind == K_NONE) return ERR_DECODE;
+                        if (get_bytes(C[DS_QS], qual, cr.len)) return ERR_DECODE;
+                    }
                 } else W::fill(qual, 255, (uint32_t)cr.len);
             }
-            if (!T->qs_seq_orient && (cr.flags & BAM_FREVERSE)) {
+            if (!T->qs_seq_orient && (ds & CRAM_QS) && (cr.flags & BAM_FREVERSE)) {
                 W::sync();
                 for (int32_t i = 0, j = cr.len - 1; i < j; i++, j--) { const uint8_t c = qual[i]; qual[i] = qual[j]; qual[j] = c; }
                 W::sync();
@@ -841,9 +927,13 @@ struct SliceDec {
     }
 };
 
-// cram_decode_slice_xref :2140-2304 (all fields required).  Serial over the slice's records.
-CRAMREC_HD inline int slice_xref(Rec *crecs, int32_t n)
+// cram_decode_slice_xref :2140-2304.  Serial over the slice's records.
+CRAMREC_HD inline int slice_xref(Rec *crecs, int32_t n, int32_t req)
 {
+    if (!(req & (SAM_RNEXT | SAM_PNEXT | SAM_TLEN))) {
+        for (int32_t rec = 0; rec < n; rec++) { crecs[rec].tlen = 0; crecs[rec].mate_pos = 0; crecs[rec].mate_ref_id = -1; }
+        return 0;
+    }
     for (int32_t rec = 0; rec < n; rec++) {
         Rec *cr = &crecs[rec];
         if (cr->mate_line >= 0) {
@@ -910,7 +1000,7 @@ CRAMREC_HD inline int reg2bin(int64_t beg, int64_t end)                   // hts
 }
 CRAMREC_HD inline int count_digits(uint64_t v) { int n = 1; while (v >= 10) { v /= 10; n++; } return n; }
 
-struct NameInfo { uint32_t len; int from_mate; uint64_t number; };        // how the QNAME of a record is made
+struct NameInfo { uint32_t len; int from_mate; uint64_t number; };        // how the QNAME of a record is made (from_mate 3: "?")
 CRAMREC_HD inline NameInfo name_info(const Rec *crecs, int32_t n, int32_t rec, uint32_t prefix_len, int64_t record_counter)
 {
     const Rec &cr = crecs[rec];
@@ -923,18 +1013,26 @@ CRAMREC_HD inline NameInfo name_info(const Rec *crecs, int32_t n, int32_t rec, u
     return ni;
 }
 
+// cram_to_bam :3110-3166: QNAME is "?" without SAM_QNAME, SEQ "*" (length 0) without SAM_SEQ and SAM_QUAL
+CRAMREC_HD inline uint32_t qname_len(const Rec *crecs, int32_t n, int32_t rec, uint32_t prefix_len, int64_t record_counter, int32_t req)
+{
+    return (req & SAM_QNAME) ? name_info(crecs, n, rec, prefix_len, record_counter).len : 1;
+}
+CRAMREC_HD inline int32_t bam_len(const Rec &cr, int32_t req) { return (req & (SAM_SEQ | SAM_QUAL)) ? cr.len : 0; }
+
 // l_data of record `rec`, or -1 where cram_to_bam / bam_set1 fail
 CRAMREC_HD inline int64_t bam_size(const Rec *crecs, int32_t n, int32_t rec, uint32_t prefix_len, int64_t record_counter,
-                                   const uint32_t *rg_len, int32_t nrg)
+                                   const uint32_t *rg_len, int32_t nrg, int32_t req)
 {
     const Rec &cr = crecs[rec];
     if (cr.rg < -1 || cr.rg >= nrg) return -1;
-    uint32_t lq = name_info(crecs, n, rec, prefix_len, record_counter).len;
+    uint32_t lq = qname_len(crecs, n, rec, prefix_len, record_counter, req);
     if (lq == 0) lq = 1;
     if (lq > 254) return -1;
     const uint32_t nuls = 4 - lq % 4;
     const uint32_t rgl = cr.rg != -1 ? rg_len[cr.rg] + 4 : 0;
-    return (int64_t)lq + nuls + (int64_t)cr.ncigar * 4 + ((int64_t)cr.len + 1) / 2 + cr.len + cr.aux_size + rgl;
+    const int64_t len = bam_len(cr, req);
+    return (int64_t)lq + nuls + (int64_t)cr.ncigar * 4 + (len + 1) / 2 + len + cr.aux_size + rgl;
 }
 
 CRAMREC_HD inline uint8_t nt16_of(uint8_t c)                              // seq_nt16_table, hts.c
@@ -963,10 +1061,12 @@ CRAMREC_HD inline uint8_t nt16_of(uint8_t c)                              // seq
 template <class W>
 CRAMREC_HD inline int bam_fill(const Rec *crecs, int32_t n, int32_t rec, const uint8_t *prefix, uint32_t prefix_len, int64_t record_counter,
                                const uint8_t *name_blk, const uint8_t *seqs, const uint8_t *quals, const uint8_t *aux_blk, const uint32_t *cigars,
-                               const uint8_t *rg_names, const uint32_t *rg_off, const uint32_t *rg_len, BamCore &core, uint8_t *data)
+                               const uint8_t *rg_names, const uint32_t *rg_off, const uint32_t *rg_len, int32_t req, BamCore &core, uint8_t *data)
 {
     const Rec &cr = crecs[rec];
-    const NameInfo ni = name_info(crecs, n, rec, prefix_len, record_counter);
+    NameInfo ni = name_info(crecs, n, rec, prefix_len, record_counter);
+    if (!(req & SAM_QNAME)) { ni.len = 1; ni.from_mate = 3; }
+    const int32_t len = bam_len(cr, req);
     uint32_t lq = ni.len;
     const bool star = lq == 0;
     if (star) lq = 1;
@@ -982,14 +1082,15 @@ CRAMREC_HD inline int bam_fill(const Rec *crecs, int32_t n, int32_t rec, const u
         }
     }
     if (rlen == 0) rlen = 1;
-    if (!(cr.flags & BAM_FUNMAP) && cr.len > 0 && cr.ncigar == 0) return -1;
-    if (!(cr.flags & BAM_FUNMAP) && cr.len > 0 && cr.len != qlen) return -1;
+    if (!(cr.flags & BAM_FUNMAP) && len > 0 && cr.ncigar == 0) return -1;
+    if (!(cr.flags & BAM_FUNMAP) && len > 0 && len != qlen) return -1;
     core.pos = cr.apos - 1; core.tid = cr.ref_id; core.bin = (uint16_t)reg2bin(cr.apos - 1, cr.apos - 1 + rlen);
     core.qual = (uint8_t)cr.mqual; core.l_extranul = (uint8_t)(nuls - 1); core.flag = (uint16_t)cr.flags;
-    core.l_qname = (uint16_t)(lq + nuls); core.n_cigar = cr.ncigar; core.l_qseq = cr.len;
+    core.l_qname = (uint16_t)(lq + nuls); core.n_cigar = cr.ncigar; core.l_qseq = len;
     core.mtid = cr.mate_ref_id; core.mpos = cr.mate_pos - 1; core.isize = cr.tlen;
     uint8_t *cp = data;
     if (star) cp[0] = '*';
+    else if (ni.from_mate == 3) cp[0] = '?';
     else if (ni.from_mate == 0) W::copy(cp, name_blk + cr.name, lq);
     else if (ni.from_mate == 1) W::copy(cp, name_blk + crecs[cr.mate_line].name, lq);
     else {
@@ -1003,10 +1104,11 @@ CRAMREC_HD inline int bam_fill(const Rec *crecs, int32_t n, int32_t rec, const u
     W::copy(cp, reinterpret_cast<const uint8_t *>(cig), cr.ncigar * 4);
     cp += cr.ncigar * 4;
     const uint8_t *sq = seqs + cr.seq;
-    W::pack_seq(cp, sq, (uint32_t)cr.len);
-    cp += (cr.len + 1) / 2;
-    W::copy(cp, quals + cr.qual, (uint32_t)cr.len);
-    cp += cr.len;
+    W::pack_seq(cp, sq, (uint32_t)len);
+    cp += (len + 1) / 2;
+    if (req & SAM_QUAL) W::copy(cp, quals + cr.qual, (uint32_t)len);
+    else W::fill(cp, 0xff, (uint32_t)len);
+    cp += len;
     W::copy(cp, aux_blk + cr.aux, cr.aux_size);
     cp += cr.aux_size;
     if (cr.rg != -1) {

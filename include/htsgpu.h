@@ -538,6 +538,43 @@ int hgpu_cram_decode_records_dev(hgpu_ctx *ctx, const uint8_t *file, uint64_t fi
  * (BZIP2 / LZMA) fails the call with that block's status. */
 int hgpu_cram_decode_file_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_refs *refs,
                                const char *name_prefix, int decode_md, hgpu_cram_records *out);
+/* Only some fields of every record — CRAM_OPT_REQUIRED_FIELDS (cram_dependent_data_series, cram/cram_decode.c:553-869, and
+ * the ~100 data-series gates of cram_decode_slice / cram_decode_seq / cram_decode_aux / cram_decode_slice_xref / cram_to_bam).
+ * required_fields: HGPU_SAM_* bits as htslib's SAM_* (hts.h:279-291); 0 and HGPU_SAM_ALL read every series, and 0 then
+ * builds the records as for a mask naming no field, as the reference does (cram_to_bam tests the mask itself).  Per slice the
+ * fields select the data series to read and the external blocks those series (and any series or tag sharing a block with
+ * them) read; the record loop skips every other series.  The result is what sam_read1 returns after hts_set_opt(fp,
+ * CRAM_OPT_REQUIRED_FIELDS, required_fields): QNAME "?" without QNAME, SEQ "*" without SEQ and QUAL, no qualities without
+ * QUAL, mate fields reset without RNEXT / PNEXT / TLEN, MD / NM not generated without AUX; fields nobody asked for hold
+ * whatever the reference leaves there.  Without SEQ no external reference is read (refs may be NULL). */
+#define HGPU_SAM_QNAME 0x00000001
+#define HGPU_SAM_FLAG  0x00000002
+#define HGPU_SAM_RNAME 0x00000004
+#define HGPU_SAM_POS   0x00000008
+#define HGPU_SAM_MAPQ  0x00000010
+#define HGPU_SAM_CIGAR 0x00000020
+#define HGPU_SAM_RNEXT 0x00000040
+#define HGPU_SAM_PNEXT 0x00000080
+#define HGPU_SAM_TLEN  0x00000100
+#define HGPU_SAM_SEQ   0x00000200
+#define HGPU_SAM_QUAL  0x00000400
+#define HGPU_SAM_AUX   0x00000800
+#define HGPU_SAM_RGAUX 0x00001000
+#define HGPU_SAM_ALL   0x7fffffff
+/* which blocks a decode of required_fields reads, host only.  Needs only the header blocks (content types 0 / 1 / 2)
+ * uncompressed in udata + udata_off[i].  used[i] (n_blocks entries) = 1 for the header blocks, the CORE block of every slice,
+ * an embedded reference block and every external block a selected series or tag reads; every block outside subset mode.
+ * Returns the number of used blocks, or -1 (a malformed compression or slice header). */
+long hgpu_cram_required_blocks(const hgpu_cram_block *blocks, uint32_t n_blocks, const uint8_t *udata, const uint64_t *udata_off,
+                               uint32_t required_fields, uint8_t *used);
+/* hgpu_cram_decode_records_host for a field subset: blocks with used == 0 may hold anything in udata. */
+int hgpu_cram_decode_records_fields_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len,
+        const hgpu_cram_block *blocks, uint32_t n_blocks, const uint8_t *udata, const uint64_t *udata_off,
+        const hgpu_cram_refs *refs, const char *name_prefix, int decode_md, uint32_t required_fields, hgpu_cram_records *out);
+/* hgpu_cram_decode_file_host for a field subset: the header blocks are uncompressed first, then only the used blocks, so an
+ * unused block is neither uncompressed nor CRC-checked (a damaged one does not fail the call), as in the reference. */
+int hgpu_cram_decode_file_fields_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_refs *refs,
+                                      const char *name_prefix, int decode_md, uint32_t required_fields, hgpu_cram_records *out);
 /* device time (CUDA events) of cram_slice_decode_kernel and cram_bam_fill_kernel in the last record-decode call: measurement only */
 void hgpu_cram_records_last_ms(float *slice_decode_ms, float *bam_fill_ms);
 

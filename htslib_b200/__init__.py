@@ -520,6 +520,33 @@ def cram_decode_records(ctx, file_np, blocks, udata, udata_off, fasta=None, pref
     return _records_out(out, free)
 
 
+CRAM_ENC_ATTACH_MATES = 0x1          # HGPU_CRAM_ENC_ATTACH_MATES
+
+
+def cram_encode_records(ctx, header_text, core, data, data_off, n, fasta=None, records_per_slice=0, minor_version=1, enc_flags=0):
+    """hgpu_cram_encode_records_opts_host: n bam1_t records (core: BAM1_CORE_DT array, data: uint8, data_off: uint64 n + 1)
+    -> a CRAM 3.x file image (bytes).  fasta: load_fasta_upper's (bases, offsets) in @SQ order, or None."""
+    L = lib()
+    refs, keep = _cram_refs(fasta)
+    L.hgpu_cram_encode_records_opts_host.argtypes = [C.c_void_p, C.c_char_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
+                                                     C.c_void_p, C.c_uint32, C.c_int, C.c_uint32, C.c_void_p, C.c_void_p]
+    out, ln = C.c_void_p(), C.c_uint64(0)
+    rc = L.hgpu_cram_encode_records_opts_host(ctx.h, header_text, len(header_text), core.ctypes.data, data.ctypes.data, data_off.ctypes.data, n,
+                                              refs, records_per_slice, minor_version, enc_flags, C.byref(out), C.byref(ln))
+    if rc != 0:
+        raise HgpuError("cram_encode_records: %d %s" % (rc, last_error()))
+    img = C.string_at(out.value, ln.value)
+    C.CDLL(None).free(C.c_void_p(out.value))
+    return img
+
+
+def cram_encode_last_ms():
+    """(pairing kernels, count + scan + write kernels) device ms of the last cram_encode_records call."""
+    a, b = C.c_float(0), C.c_float(0)
+    lib().hgpu_cram_encode_last_ms(C.byref(a), C.byref(b))
+    return a.value, b.value
+
+
 # CRAM_OPT_REQUIRED_FIELDS bits (htslib's SAM_*, hts.h:279-291; HGPU_SAM_* in htsgpu.h)
 SAM_QNAME, SAM_FLAG, SAM_RNAME, SAM_POS, SAM_MAPQ, SAM_CIGAR, SAM_RNEXT = 0x1, 0x2, 0x4, 0x8, 0x10, 0x20, 0x40
 SAM_PNEXT, SAM_TLEN, SAM_SEQ, SAM_QUAL, SAM_AUX, SAM_RGAUX, SAM_ALL = 0x80, 0x100, 0x200, 0x400, 0x800, 0x1000, 0x7fffffff

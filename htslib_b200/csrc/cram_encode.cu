@@ -7,7 +7,9 @@
 // then compressed by the existing device encoders — the method trial of hgpu_cram_compress_blocks_host for every series
 // (rANS Nx16 family for CRAM 3.1, rANS 4x8 for 3.0) and the tok3 encoder for read names (3.1) — and framed with the
 // device CRC-32.  Host: the tag dictionary (one walk over the aux field headers), compression / slice / container headers.
-// One slice per container; slices are independent, which is the axis that shards across GPUs.
+// One slice per container; slices are independent, which is the axis that shards across GPUs.  With mate attachment
+// the pairing kernels (cram_mate_key / group / scan / fill / resolve) run first and hand walk() each record's CF bits
+// and NF (see cram_encode.cuh).
 //
 // Built a second time by tests/hostsim (-DHGPU_HOSTSIM): kernels -> loops, blocks stored RAW (the codecs are GPU-only);
 // the reference must read that file back to the input records.  libhtsgpu.so never contains that variant.
@@ -27,6 +29,10 @@ struct hgpu_ctx;
 #include <map>
 #include <string>
 #include <vector>
+#ifdef HGPU_HOSTSIM
+static std::vector<uint8_t> g_mate_cf;             // the pairing pass's decisions of the last call with mate attachment
+static std::vector<int32_t> g_mate_nf;
+#endif
 #include <stdlib.h>
 #include <string.h>
 
@@ -73,7 +79,7 @@ void frame_block(Buf &o, int method, int ctype, int32_t cid, const uint8_t *payl
 }
 
 const char *const k_keys[S_COUNT] = {"BF", "CF", "RI", "RL", "AP", "RG", "RN", "MF", "NS", "NP", "TS", "TL", "FN", "FC", "FP", "DL", "RS", "HC", "PD",
-                                     nullptr, "BB", nullptr, "SC", nullptr, "IN", "BA", "QS", "MQ", nullptr, nullptr, "BS"};
+                                     nullptr, "BB", nullptr, "SC", nullptr, "IN", "BA", "QS", "MQ", nullptr, nullptr, "BS", "NF"};
 
 void enc_external(Buf &o, int id) { o.itf8(1); Buf t; t.itf8(id); o.itf8((int32_t)t.v.size()); o.bytes(t.v.data(), t.v.size()); }
 void enc_byte_array_len(Buf &o, int len_id, int val_id)
@@ -85,7 +91,7 @@ void enc_byte_array_len(Buf &o, int len_id, int val_id)
 }
 
 // cram_encode_compression_header :380-1030 for this writer's fixed layout
-void compression_header(Buf &o, const std::vector<std::string> &tag_lines, const std::vector<uint32_t> &tag_keys, bool ref_required)
+void compression_header(Buf &o, const std::vector<std::string> &tag_lines, const std::vector<uint32_t> &tag_keys, bool ref_required, bool attach)
 {
     Buf pm;                                                                // preservation map
     pm.itf8(5);
@@ -101,7 +107,7 @@ void compression_header(Buf &o, const std::vector<std::string> &tag_lines, const
     int cnt = 0;
     Buf body;
     for (int s = 0; s < S_COUNT; s++) {
-        if (!k_keys[s]) continue;
+        if (!k_keys[s] || (s == S_NF && !attach)) continue;
         body.u8((uint8_t)k_keys[s][0]); body.u8((uint8_t)k_keys[s][1]);
         if (s == S_RN) { body.itf8(5); Buf t; t.u8(0); t.itf8(s + 1); body.itf8((int32_t)t.v.size()); body.bytes(t.v.data(), t.v.size()); }
         else if (s == S_BB || s == S_SC || s == S_IN) enc_byte_array_len(body, s, s + 1);              // the length stream sits just before its value stream
@@ -125,7 +131,122 @@ struct EArgs {
     const uint64_t *base;                   // [slice][stream] -> byte offset in arena
     uint8_t *arena;
     int32_t *status;                        // per record
+    const uint8_t *mate_cf;                 // per record: the pairing pass's CF bits (nullptr: every record detached)
+    const int32_t *mate_nf;                 // per record: NF of MATE_DOWNSTREAM records
 };
+
+// the pairing pass: key (hash, aend) -> group (open-addressing name table per slice) -> scan of the group sizes ->
+// member lists -> resolve (one thread per group replays process_one_read's rule in record order)
+struct PArgs {
+    const Core *core; const uint8_t *data; const uint64_t *data_off;
+    const uint64_t *ref_off; int32_t n_ref; bool no_ref;
+    uint64_t n; uint32_t rps, tsize;        // records, records per slice, table slots per slice (a power of two >= 2 rps)
+    uint64_t *hash; int64_t *aend;          // per record
+    int32_t *slot;                          // [slice][tsize]: slice-local record number of the slot's first read, -1 = free
+    uint32_t *gcnt, *gstart, *gfill;        // [slice][tsize]: reads per slot, their first place in mem, places taken
+    int32_t *grp;                           // per record: its slot, -1 = not paired
+    uint32_t *mem;                          // [slice][rps]: slice-local record numbers, grouped by slot
+    uint8_t *cf; int32_t *nf;               // per record: decisions
+    uint64_t hash_mask;
+};
+
+#ifdef HGPU_HOSTSIM
+static uint64_t g_hash_mask = ~0ull;        // tests force collisions with a narrower mask
+#endif
+// atomics on the device; the host build runs the kernels as serial loops
+CRAMREC_HD inline int32_t at_cas(int32_t *p, int32_t cmp, int32_t v)
+{
+#ifdef __CUDA_ARCH__
+    return atomicCAS(p, cmp, v);
+#else
+    const int32_t o = *p; if (o == cmp) *p = v; return o;
+#endif
+}
+CRAMREC_HD inline uint32_t at_add(uint32_t *p, uint32_t v)
+{
+#ifdef __CUDA_ARCH__
+    return atomicAdd(p, v);
+#else
+    const uint32_t o = *p; *p += v; return o;
+#endif
+}
+
+// c->ref_end when process_one_read sees record g (cram_encode.c:1923-1927, :2037-2056): with a reference, the length of the
+// sequence of the last record of the container (= slice here) up to g whose reference id is set; 0 before any, and 0
+// throughout without a reference
+CRAMREC_HD inline int64_t mate_ref_end(const PArgs &A, uint64_t g)
+{
+    if (A.no_ref) return 0;
+    const uint64_t first = g / A.rps * A.rps;
+    for (uint64_t r = g + 1; r-- > first;) {
+        const int32_t t = A.core[r].tid;
+        if (t >= 0 && t < A.n_ref) return (int64_t)(A.ref_off[t + 1] - A.ref_off[t]);
+    }
+    return 0;
+}
+
+CRAMREC_HD inline uint32_t rec_name_len(const PArgs &A, uint64_t g)
+{
+    const uint64_t l = A.data_off[g + 1] - A.data_off[g];
+    return mate_name_len(A.data + A.data_off[g], A.core[g].l_qname < l ? A.core[g].l_qname : (uint32_t)l);
+}
+
+CRAMREC_HD inline void key_body(const PArgs &A, uint64_t g)
+{
+    const Core &c = A.core[g];
+    A.cf[g] = MATE_DETACHED; A.nf[g] = 0;
+    // an unmapped read at apos <= 0 ends at apos whatever ref_end is (>= 0): skip the walk back for the unplaced tail
+    const int64_t re = (c.flag & 4) && c.pos + 1 <= 0 ? 0 : mate_ref_end(A, g);
+    A.aend[g] = mate_aend(c, A.data + A.data_off[g], (uint32_t)(A.data_off[g + 1] - A.data_off[g]), A.no_ref, re);
+    A.hash[g] = mate_hash(A.data + A.data_off[g], rec_name_len(A, g), (c.flag & 0x100) != 0) & A.hash_mask;
+}
+
+CRAMREC_HD inline bool same_name(const PArgs &A, uint64_t a, uint64_t b)
+{
+    if (A.hash[a] != A.hash[b] || ((A.core[a].flag ^ A.core[b].flag) & 0x100)) return false;
+    const uint32_t la = rec_name_len(A, a), lb = rec_name_len(A, b);
+    if (la != lb) return false;
+    const uint8_t *pa = A.data + A.data_off[a], *pb = A.data + A.data_off[b];
+    for (uint32_t i = 0; i < la; i++) if (pa[i] != pb[i]) return false;
+    return true;
+}
+
+CRAMREC_HD inline void group_body(const PArgs &A, uint64_t g)
+{
+    if (!(A.core[g].flag & 1)) { A.grp[g] = -1; return; }
+    const uint64_t sl = g / A.rps, g0 = sl * A.rps;
+    int32_t *slot = A.slot + sl * A.tsize;
+    uint32_t s = (uint32_t)A.hash[g] & (A.tsize - 1);
+    for (;;) {                                     // the table has 2 slots per read of the slice: a free one is always found
+        const int32_t cur = at_cas(&slot[s], -1, (int32_t)(g - g0));
+        if (cur < 0 || same_name(A, g0 + (uint32_t)cur, g)) break;
+        s = (s + 1) & (A.tsize - 1);
+    }
+    A.grp[g] = (int32_t)s;
+    at_add(&A.gcnt[sl * A.tsize + s], 1);
+}
+
+CRAMREC_HD inline void fill_body(const PArgs &A, uint64_t g)
+{
+    if (A.grp[g] < 0) return;
+    const uint64_t sl = g / A.rps, row = sl * A.tsize + (uint32_t)A.grp[g];
+    A.mem[sl * A.rps + A.gstart[row] + at_add(&A.gfill[row], 1)] = (uint32_t)(g - sl * A.rps);
+}
+
+CRAMREC_HD inline void resolve_body(const PArgs &A, uint64_t row)
+{
+    const uint32_t k = A.gcnt[row];
+    if (k < 2) return;
+    const uint64_t sl = row / A.tsize, g0 = sl * A.rps;
+    uint32_t *m = A.mem + g0 + A.gstart[row];
+    for (uint32_t i = 1; i < k; i++) {             // record order (the fill pass placed them in any order); groups are tiny
+        const uint32_t v = m[i];
+        uint32_t j = i;
+        for (; j > 0 && m[j - 1] > v; j--) m[j] = m[j - 1];
+        m[j] = v;
+    }
+    mate_replay(m, k, A.core + g0, A.aend + g0, A.cf + g0, A.nf + g0);
+}
 
 CRAMREC_HD inline void count_body(const EArgs &A, uint64_t g)
 {
@@ -135,7 +256,8 @@ CRAMREC_HD inline void count_body(const EArgs &A, uint64_t g)
     Emit<false> E{n, nullptr};
     const uint8_t *ref = nullptr; int64_t rl = 0;
     if (A.ref_bases && A.core[g].tid >= 0 && A.core[g].tid < A.n_ref) { ref = A.ref_bases + A.ref_off[A.core[g].tid]; rl = (int64_t)(A.ref_off[A.core[g].tid + 1] - A.ref_off[A.core[g].tid]); }
-    const int rc = walk<false>(A.core[g], A.data + A.data_off[g], (uint32_t)(A.data_off[g + 1] - A.data_off[g]), A.tl[g], ref, rl, E);
+    const int rc = walk<false>(A.core[g], A.data + A.data_off[g], (uint32_t)(A.data_off[g + 1] - A.data_off[g]), A.tl[g], ref, rl,
+                               A.mate_cf ? A.mate_cf[g] : MATE_DETACHED, A.mate_nf ? A.mate_nf[g] : 0, E);
     A.status[g] = rc;
     for (int s = 0; s < S_COUNT; s++) A.cnt[((size_t)sl * S_COUNT + s) * A.rps + r] = rc == ENC_OK ? n[s] : 0;
 }
@@ -150,7 +272,8 @@ CRAMREC_HD inline void write_body(const EArgs &A, uint64_t g)
     Emit<true> E{n, base};
     const uint8_t *ref = nullptr; int64_t rl = 0;
     if (A.ref_bases && A.core[g].tid >= 0 && A.core[g].tid < A.n_ref) { ref = A.ref_bases + A.ref_off[A.core[g].tid]; rl = (int64_t)(A.ref_off[A.core[g].tid + 1] - A.ref_off[A.core[g].tid]); }
-    walk<true>(A.core[g], A.data + A.data_off[g], (uint32_t)(A.data_off[g + 1] - A.data_off[g]), A.tl[g], ref, rl, E);
+    walk<true>(A.core[g], A.data + A.data_off[g], (uint32_t)(A.data_off[g + 1] - A.data_off[g]), A.tl[g], ref, rl,
+               A.mate_cf ? A.mate_cf[g] : MATE_DETACHED, A.mate_nf ? A.mate_nf[g] : 0, E);
 }
 
 #ifndef HGPU_HOSTSIM
@@ -183,11 +306,54 @@ __global__ void __launch_bounds__(128) cram_enc_write_kernel(EArgs A)
     const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g < A.n) write_body(A, g);
 }
+
+float g_enc_ms[2] = {0, 0};                    // device time of the last call: pairing kernels, count + scan + write kernels
+__global__ void __launch_bounds__(128) cram_mate_key_kernel(PArgs A)
+{
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g < A.n) key_body(A, g);
+}
+__global__ void __launch_bounds__(128) cram_mate_group_kernel(PArgs A)
+{
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g < A.n) group_body(A, g);
+}
+// one warp per slice: exclusive scan of the slot sizes -> each slot's first place in the slice's member list
+__global__ void __launch_bounds__(128) cram_mate_scan_kernel(PArgs A, uint32_t ns)
+{
+    const uint32_t sl = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (sl >= ns) return;
+    const uint32_t *c = A.gcnt + (size_t)sl * A.tsize;
+    uint32_t *o = A.gstart + (size_t)sl * A.tsize;
+    uint32_t run = 0;
+    for (uint32_t b = 0; b < A.tsize; b += 32) {
+        const uint32_t v = c[b + lane];
+        uint32_t inc = v;
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= (uint32_t)d) inc += t; }
+        o[b + lane] = run + inc - v;
+        run += __shfl_sync(0xffffffffu, inc, 31);
+    }
+}
+__global__ void __launch_bounds__(128) cram_mate_fill_kernel(PArgs A)
+{
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g < A.n) fill_body(A, g);
+}
+__global__ void __launch_bounds__(128) cram_mate_resolve_kernel(PArgs A, uint64_t rows)
+{
+    const uint64_t row = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (row < rows) resolve_body(A, row);
+}
 #endif
 
 int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, const hgpu_bam1_core *core, const uint8_t *data,
-                const uint64_t *data_off, uint64_t n, const hgpu_cram_refs *refs, uint32_t rps, int minor, uint8_t **out_file, uint64_t *out_len)
+                const uint64_t *data_off, uint64_t n, const hgpu_cram_refs *refs, uint32_t rps, int minor, uint32_t enc_flags,
+                uint8_t **out_file, uint64_t *out_len)
 {
+    const bool attach = (enc_flags & HGPU_CRAM_ENC_ATTACH_MATES) != 0;
+#ifdef HGPU_HOSTSIM
+    g_mate_cf.clear(); g_mate_nf.clear();
+#endif
     // reference-based shape only when every mapped record's reference sequence was supplied (the reader will need them all)
     bool use_ref = refs && refs->bases && refs->off && refs->n_ref > 0;
     if (use_ref)
@@ -200,6 +366,8 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
     *out_file = nullptr; *out_len = 0;
     if (rps == 0) rps = 10000;
     if (minor != 0 && minor != 1) { hgpu_set_error("cram encode: CRAM 3.0 or 3.1"); return HGPU_ERR_ARG; }
+    if (enc_flags & ~(uint32_t)HGPU_CRAM_ENC_ATTACH_MATES) { hgpu_set_error("cram encode: unknown flags 0x%x", enc_flags); return HGPU_ERR_ARG; }
+    if (attach && rps > (1u << 29)) { hgpu_set_error("cram encode: records per slice above 2^29 with mate attachment"); return HGPU_ERR_ARG; }
     const uint32_t ns = (uint32_t)((n + rps - 1) / rps);
     // ---- tag dictionary per slice (host: one walk over the aux field headers) ----
     std::vector<int32_t> tl(n ? n : 1, 0);
@@ -244,6 +412,13 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         // every series byte comes from the record data, ITF8 at most 5 bytes per value: bound the arena before the scan
         const size_t arena_cap = StageLayout::align(2 * data_bytes + 200 * n + 4096);
         const auto s_arena = L.seg(arena_cap);
+        // the pairing pass (mate attachment only): 2 table slots or more per read of a slice
+        uint32_t tsize = 0;
+        if (attach) { tsize = 32; while (tsize < 2 * rps) tsize <<= 1; }
+        const size_t slots = attach ? (size_t)ns * tsize : 0, nm = attach ? n : 0;
+        const auto s_hash = L.seg(nm * 8), s_aend = L.seg(nm * 8), s_mcf = L.seg(nm), s_mnf = L.seg(nm * 4), s_grp = L.seg(nm * 4),
+                   s_mem = L.seg(attach ? (size_t)ns * rps * 4 : 0), s_slot = L.seg(slots * 4), s_gcnt = L.seg(slots * 4),
+                   s_gstart = L.seg(slots * 4), s_gfill = L.seg(slots * 4);
 #ifdef HGPU_HOSTSIM
         (void)ctx;
         std::vector<uint8_t> image(L.total);
@@ -268,7 +443,29 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         A.ref_bases = use_ref ? L.at(s_ref) : nullptr; A.ref_off = L.at<uint64_t>(s_roff); A.n_ref = use_ref ? refs->n_ref : 0;
         A.cnt = L.at<uint32_t>(s_cnt); A.tot = L.at<uint32_t>(s_tot);
         A.base = L.at<uint64_t>(s_base); A.arena = L.at(s_arena); A.status = L.at<int32_t>(s_st);
+        A.mate_cf = attach ? L.at(s_mcf) : nullptr; A.mate_nf = attach ? L.at<int32_t>(s_mnf) : nullptr;
+        PArgs P;
+        P.core = A.core; P.data = A.data; P.data_off = A.data_off;
+        P.ref_off = A.ref_off; P.n_ref = A.n_ref; P.no_ref = !use_ref;
+        P.n = n; P.rps = rps; P.tsize = tsize;
+        P.hash = L.at<uint64_t>(s_hash); P.aend = L.at<int64_t>(s_aend); P.slot = L.at<int32_t>(s_slot);
+        P.gcnt = L.at<uint32_t>(s_gcnt); P.gstart = L.at<uint32_t>(s_gstart); P.gfill = L.at<uint32_t>(s_gfill);
+        P.grp = L.at<int32_t>(s_grp); P.mem = L.at<uint32_t>(s_mem); P.cf = L.at(s_mcf); P.nf = L.at<int32_t>(s_mnf);
+        P.hash_mask = ~0ull;
 #ifdef HGPU_HOSTSIM
+        if (attach) {
+            P.hash_mask = g_hash_mask;
+            memset(P.slot, 0xff, slots * 4); memset(P.gcnt, 0, slots * 4); memset(P.gfill, 0, slots * 4);
+            for (uint64_t g = 0; g < n; g++) key_body(P, g);
+            for (uint64_t g = 0; g < n; g++) group_body(P, g);
+            for (uint32_t sl = 0; sl < ns; sl++) {
+                uint32_t run = 0;
+                for (uint32_t s = 0; s < tsize; s++) { P.gstart[(size_t)sl * tsize + s] = run; run += P.gcnt[(size_t)sl * tsize + s]; }
+            }
+            for (uint64_t g = 0; g < n; g++) fill_body(P, g);
+            for (size_t row = 0; row < slots; row++) resolve_body(P, row);
+            g_mate_cf.assign(P.cf, P.cf + n); g_mate_nf.assign(P.nf, P.nf + n);
+        }
         for (uint64_t g = 0; g < n; g++) count_body(A, g);
         for (size_t row = 0; row < rows; row++) {
             const uint64_t first = (uint64_t)(row / S_COUNT) * rps;
@@ -280,8 +477,30 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         memcpy(tot.data(), A.tot, rows * 4);
         memcpy(status.data(), A.status, n * 4);
 #else
-        cram_enc_count_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A);
+        struct Events {                                  // destroyed on every return path
+            cudaEvent_t e[6]; int n = 0;
+            bool make() { for (; n < 6; n++) if (cudaEventCreate(&e[n]) != cudaSuccess) return false; return true; }
+            ~Events() { for (int k = 0; k < n; k++) cudaEventDestroy(e[k]); }
+        } evs;
+        if (!evs.make()) return HGPU_ERR_CUDA;
+        cudaEvent_t *ev = evs.e;
+        const unsigned rec_blocks = (unsigned)((n + 127) / 128);
+        cudaEventRecord(ev[0], st);
+        if (attach) {
+            if (hgpu_memset(P.slot, 0xff, slots * 4, st) || hgpu_memset(P.gcnt, 0, slots * 4, st) || hgpu_memset(P.gfill, 0, slots * 4, st)) return HGPU_ERR_CUDA;
+            cram_mate_key_kernel<<<rec_blocks, 128, 0, st>>>(P);
+            cram_mate_group_kernel<<<rec_blocks, 128, 0, st>>>(P);
+            cram_mate_scan_kernel<<<(ns + 3) / 4, 128, 0, st>>>(P, ns);
+            cram_mate_fill_kernel<<<rec_blocks, 128, 0, st>>>(P);
+            cram_mate_resolve_kernel<<<(unsigned)((slots + 127) / 128), 128, 0, st>>>(P, (uint64_t)slots);
+            hgpu_count_launch(5);
+            if (hgpu_check(cudaGetLastError(), "cram encode pairing launch")) return HGPU_ERR_CUDA;
+        }
+        cudaEventRecord(ev[1], st);
+        cudaEventRecord(ev[2], st);
+        cram_enc_count_kernel<<<rec_blocks, 128, 0, st>>>(A);
         cram_enc_scan_kernel<<<(unsigned)((rows + 3) / 4), 128, 0, st>>>(A, (uint32_t)rows);
+        cudaEventRecord(ev[3], st);
         hgpu_count_launch(2);
         if (hgpu_check(cudaGetLastError(), "cram encode launch")) return HGPU_ERR_CUDA;
         if (hgpu_d2h(tot.data(), A.tot, rows * 4, st) || hgpu_d2h(status.data(), A.status, n * 4, st) ||
@@ -303,11 +522,18 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         memcpy(arena_h.data(), A.arena, at);
 #else
         if (hgpu_h2d(L.at(s_base), base.data(), rows * 8, st)) return HGPU_ERR_CUDA;
+        cudaEventRecord(ev[4], st);
         cram_enc_write_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A);
+        cudaEventRecord(ev[5], st);
         hgpu_count_launch();
         if (hgpu_check(cudaGetLastError(), "cram encode write launch")) return HGPU_ERR_CUDA;
         if (hgpu_d2h(arena_h.data(), A.arena, at, st)) return HGPU_ERR_CUDA;
         if (hgpu_check(cudaStreamSynchronize(st), "cram encode write")) return HGPU_ERR_CUDA;
+        float cs = 0, wr = 0;
+        cudaEventElapsedTime(&g_enc_ms[0], ev[0], ev[1]);
+        cudaEventElapsedTime(&cs, ev[2], ev[3]);
+        cudaEventElapsedTime(&wr, ev[4], ev[5]);
+        g_enc_ms[1] = cs + wr;
 #endif
     }
     // ---- compress the series blocks (device codecs) ----
@@ -400,7 +626,7 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         const uint64_t a = (uint64_t)sl * rps, b = a + rps < n ? a + rps : n;
         int64_t bases = 0;
         for (uint64_t g = a; g < b; g++) bases += core[g].l_qseq;
-        Buf ch; compression_header(ch, lines[sl], keys[sl], use_ref);
+        Buf ch; compression_header(ch, lines[sl], keys[sl], use_ref, attach);
         Buf body;
         frame_block(body, 0, 1, 0, ch.v.data(), (uint32_t)ch.v.size(), (uint32_t)ch.v.size());
         const int32_t landmark = (int32_t)body.v.size();
@@ -440,15 +666,46 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
 extern "C" int hostsim_cram_encode_records(const char *header_text, uint32_t header_len, const hgpu_bam1_core *core, const uint8_t *data,
         const uint64_t *data_off, uint64_t n, const hgpu_cram_refs *refs, uint32_t rps, int minor, uint8_t **out_file, uint64_t *out_len)
 {
-    try { return encode_impl(nullptr, header_text, header_len, core, data, data_off, n, refs, rps, minor, out_file, out_len); }
+    try { return encode_impl(nullptr, header_text, header_len, core, data, data_off, n, refs, rps, minor, 0, out_file, out_len); }
     catch (...) { hgpu_set_error("internal error"); return HGPU_ERR_NOMEM; }
 }
+extern "C" int hostsim_cram_encode_records_opts(const char *header_text, uint32_t header_len, const hgpu_bam1_core *core, const uint8_t *data,
+        const uint64_t *data_off, uint64_t n, const hgpu_cram_refs *refs, uint32_t rps, int minor, uint32_t enc_flags, uint8_t **out_file, uint64_t *out_len)
+{
+    try { return encode_impl(nullptr, header_text, header_len, core, data, data_off, n, refs, rps, minor, enc_flags, out_file, out_len); }
+    catch (...) { hgpu_set_error("internal error"); return HGPU_ERR_NOMEM; }
+}
+// test hooks: the pairing decisions of the last call with mate attachment (CF bits, NF), and the mask every name hash is
+// reduced by (0 makes every name collide, so only the name comparison keeps different names apart)
+extern "C" uint64_t hostsim_cram_enc_mates(uint8_t *cf, int32_t *nf, uint64_t cap)
+{
+    const uint64_t n = g_mate_cf.size();
+    for (uint64_t i = 0; i < n && i < cap; i++) { cf[i] = g_mate_cf[i]; nf[i] = g_mate_nf[i]; }
+    return n;
+}
+extern "C" void hostsim_cram_enc_hash_mask(uint64_t mask) { g_hash_mask = mask; }
 #else
 extern "C" int hgpu_cram_encode_records_host(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, const hgpu_bam1_core *core,
         const uint8_t *data, const uint64_t *data_off, uint64_t n, const hgpu_cram_refs *refs, uint32_t records_per_slice, int minor_version,
         uint8_t **out_file, uint64_t *out_len)
 {
-    return hgpu_abi_call([&] { return encode_impl(ctx, header_text, header_len, core, data, data_off, n, refs, records_per_slice, minor_version, out_file, out_len); },
+    return hgpu_abi_call([&] { return encode_impl(ctx, header_text, header_len, core, data, data_off, n, refs, records_per_slice, minor_version, 0,
+                                                  out_file, out_len); },
                          HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
+}
+
+extern "C" int hgpu_cram_encode_records_opts_host(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, const hgpu_bam1_core *core,
+        const uint8_t *data, const uint64_t *data_off, uint64_t n, const hgpu_cram_refs *refs, uint32_t records_per_slice, int minor_version,
+        uint32_t enc_flags, uint8_t **out_file, uint64_t *out_len)
+{
+    return hgpu_abi_call([&] { return encode_impl(ctx, header_text, header_len, core, data, data_off, n, refs, records_per_slice, minor_version,
+                                                  enc_flags, out_file, out_len); },
+                         HGPU_ERR_NOMEM, HGPU_ERR_NOMEM);
+}
+
+extern "C" void hgpu_cram_encode_last_ms(float *pair_ms, float *count_write_ms)
+{
+    if (pair_ms) *pair_ms = g_enc_ms[0];
+    if (count_write_ms) *count_write_ms = g_enc_ms[1];
 }
 #endif

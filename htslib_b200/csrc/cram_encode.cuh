@@ -11,10 +11,13 @@
 //   BF CF RI RL AP RG | RN (BYTE_ARRAY_STOP 0) | MF NS NP TS | TL | FN, per feature FC FP and DL / RS / HC / PD or
 //   BB / SC / IN (BYTE_ARRAY_LEN: length stream + value stream) | BA (unmapped reads) | QS | MQ |
 //   tags: every tag value BYTE_ARRAY_LEN over two shared streams (lengths, values), in tag-line order.
-// Every record is written detached (MF NS NP TS explicit, no mate cross references to resolve), RG stays an ordinary
-// aux tag (RG series = -1), AP is absolute, RI is per record (multi-reference slice, ref_seq_id -2) and RR = 0 (no
-// reference needed to decode).  What the reference's decoder returns for such a slice is the input record, except what
-// CRAM cannot hold: '=' / 'X' CIGAR ops come back as 'M', the mapping quality of an unmapped read as 0.
+//   NF (mate distance, only with mate attachment) comes last, content id 32, so the layout without it is unchanged.
+// By default every record is written detached (MF NS NP TS explicit, no mate cross references to resolve).  With mate
+// attachment the pairing pass below decides per record, as process_one_read does, which reads of a name are attached:
+// the earlier read gets MATE_DOWNSTREAM and NF, neither stores MF NS NP TS, the decoder rebuilds them.  RG stays an
+// ordinary aux tag (RG series = -1), AP is absolute, RI is per record (multi-reference slice, ref_seq_id -2) and RR = 0
+// (no reference needed to decode).  What the reference's decoder returns for such a slice is the input record, except
+// what CRAM cannot hold: '=' / 'X' CIGAR ops come back as 'M', the mapping quality of an unmapped read as 0.
 #pragma once
 #include <stdint.h>
 #include <stddef.h>
@@ -30,7 +33,7 @@
 namespace cramenc {
 
 enum Stream { S_BF, S_CF, S_RI, S_RL, S_AP, S_RG, S_RN, S_MF, S_NS, S_NP, S_TS, S_TL, S_FN, S_FC, S_FP, S_DL, S_RS, S_HC, S_PD,
-              S_BB_LEN, S_BB, S_SC_LEN, S_SC, S_IN_LEN, S_IN, S_BA, S_QS, S_MQ, S_TAG_LEN, S_TAG_VAL, S_BS, S_COUNT };
+              S_BB_LEN, S_BB, S_SC_LEN, S_SC, S_IN_LEN, S_IN, S_BA, S_QS, S_MQ, S_TAG_LEN, S_TAG_VAL, S_BS, S_NF, S_COUNT };
 
 struct Core { int64_t pos; int32_t tid; uint16_t bin; uint8_t qual, l_extranul; uint16_t flag, l_qname; uint32_t n_cigar; int32_t l_qseq, mtid; int64_t mpos, isize; };
 
@@ -164,9 +167,12 @@ CRAMREC_HD inline int features(const Core &c, const uint8_t *cig, uint32_t nc, c
 }
 
 // One record.  tl = its tag-line index (the host built the dictionary).  ref / ref_len: the record's reference sequence
-// (nullptr: none).  Returns ENC_OK or why the slice cannot be written here.
+// (nullptr: none).  mate_cf / mate_nf: the pairing pass's decision (MATE_DETACHED without it).  Returns ENC_OK or why
+// the slice cannot be written here.
+enum { MATE_DETACHED = 2, MATE_DOWNSTREAM = 4 };                               // CRAM_FLAG_DETACHED, CRAM_FLAG_MATE_DOWNSTREAM
 template <bool WRITE>
-CRAMREC_HD inline int walk(const Core &c, const uint8_t *data, uint32_t l_data, int32_t tl, const uint8_t *ref, int64_t ref_len, Emit<WRITE> &E)
+CRAMREC_HD inline int walk(const Core &c, const uint8_t *data, uint32_t l_data, int32_t tl, const uint8_t *ref, int64_t ref_len,
+                           uint32_t mate_cf, int32_t mate_nf, Emit<WRITE> &E)
 {
     const uint32_t lq = c.l_qname, nc = c.n_cigar;
     const int32_t ls = c.l_qseq;
@@ -188,7 +194,7 @@ CRAMREC_HD inline int walk(const Core &c, const uint8_t *data, uint32_t l_data, 
     }
     if (noseq && nc == 0) return ENC_UNSUPPORTED;
     E.put_int(S_BF, c.flag);
-    E.put_int(S_CF, 2 | (has_qual ? 1 : 0) | (noseq ? 8 : 0));               // DETACHED | PRESERVE_QUAL_SCORES | NO_SEQ
+    E.put_int(S_CF, (int32_t)mate_cf | (has_qual ? 1 : 0) | (noseq ? 8 : 0)); // DETACHED / MATE_DOWNSTREAM | PRESERVE_QUAL_SCORES | NO_SEQ
     E.put_int(S_RI, c.tid);
     E.put_int(S_RL, noseq ? (int32_t)cig_q : ls);
     E.put_int(S_AP, (int32_t)(c.pos + 1));
@@ -199,10 +205,13 @@ CRAMREC_HD inline int walk(const Core &c, const uint8_t *data, uint32_t l_data, 
         E.put_bytes(S_RN, data, nl);
         E.put_byte(S_RN, 0);
     }
-    E.put_int(S_MF, 0);
-    E.put_int(S_NS, c.mtid);
-    E.put_int(S_NP, (int32_t)(c.mpos + 1));
-    E.put_int(S_TS, (int32_t)c.isize);
+    if (mate_cf & MATE_DETACHED) {
+        E.put_int(S_MF, 0);
+        E.put_int(S_NS, c.mtid);
+        E.put_int(S_NP, (int32_t)(c.mpos + 1));
+        E.put_int(S_TS, (int32_t)c.isize);
+    }
+    if (mate_cf & MATE_DOWNSTREAM) E.put_int(S_NF, mate_nf);
     E.put_int(S_TL, tl);
     // tags: lengths + values, in order
     for (const uint8_t *p = aux; p < end;) {
@@ -223,6 +232,92 @@ CRAMREC_HD inline int walk(const Core &c, const uint8_t *data, uint32_t l_data, 
     } else E.put_bases(S_BA, seq4, 0, (uint32_t)ls);
     if (has_qual) E.put_bytes(S_QS, qual, (uint32_t)ls);
     return ENC_OK;
+}
+
+// ---- mate pairing: the mate block of process_one_read (cram_encode.c:3799-4012) for CRAM 3.x with the default options
+// (tlen_zero = tlen_approx = 0, names kept).  Per slice, BAM_FPAIRED reads go into one of two name tables, pair[sec]
+// (sec = BAM_FSECONDARY set).  The reads of one table entry form a group; groups are independent, a group's rule is
+// serial in record order (mate_replay).
+
+// 64-bit FNV-1a of the name (bam_name: up to its NUL) and the table it goes in
+CRAMREC_HD inline uint64_t mate_hash(const uint8_t *name, uint32_t len, int sec)
+{
+    uint64_t h = 0xcbf29ce484222325ull ^ (uint64_t)sec;
+    for (uint32_t i = 0; i < len; i++) h = (h ^ name[i]) * 0x100000001b3ull;
+    return h;
+}
+CRAMREC_HD inline uint32_t mate_name_len(const uint8_t *data, uint32_t l_qname) { uint32_t n = 0; while (n < l_qname && data[n]) n++; return n; }
+
+// cr->aend of process_one_read: a mapped read ends at pos + the reference bases its CIGAR spans (M D N = X), clamped to
+// the container's reference end when coded against a reference (:3718); an unmapped read "ends" at MIN(apos, ref_end)
+// (:3730).  ref_end is c->ref_end: 0 without a reference (the container is calloc'd and never given one), otherwise the
+// length of the last reference sequence loaded for the container's records (see mate_ref_end in cram_encode.cu).
+CRAMREC_HD inline int64_t mate_aend(const Core &c, const uint8_t *data, uint32_t l_data, bool no_ref, int64_t ref_end)
+{
+    const int64_t apos = c.pos + 1;
+    if (c.flag & 4) return apos < ref_end ? apos : ref_end;
+    int64_t e = c.pos;
+    const uint32_t nc = c.n_cigar;
+    if ((uint64_t)c.l_qname + 4ull * nc > l_data) return apos;                // malformed: the count pass refuses the record
+    const uint8_t *cig = data + c.l_qname;
+    for (uint32_t k = 0; k < nc; k++) {
+        const uint32_t w = cig[4 * k] | cig[4 * k + 1] << 8 | cig[4 * k + 2] << 16 | (uint32_t)cig[4 * k + 3] << 24;
+        const uint32_t op = w & 15;
+        if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) e += w >> 4;
+    }
+    if (no_ref) return e;
+    const int64_t re = ref_end > 0 ? ref_end : 0;
+    return e < re ? e : re;
+}
+
+// The state process_one_read keeps for the record a name table entry points at (cram_record's fields of those names).
+struct MateRec { int64_t apos, aend, mate_pos, tlen; int32_t ref_id; uint32_t flags, mate_flags; };
+
+CRAMREC_HD inline MateRec mate_detached(const Core &c, int64_t aend)
+{
+    MateRec m;
+    m.apos = c.pos + 1; m.aend = aend; m.ref_id = c.tid; m.flags = c.flag;
+    m.mate_flags = ((c.flag & 8) ? 2u : 0u) | ((c.flag & 0x20) ? 1u : 0u);     // CRAM_M_UNMAP, CRAM_M_REVERSE
+    m.mate_pos = c.mpos + 1 > 0 ? c.mpos + 1 : 0;
+    m.tlen = c.isize;
+    return m;
+}
+
+// One group: members[0 .. k) are global record numbers of one slice in increasing order.  cf[] / nf[] arrive as
+// MATE_DETACHED / 0 and leave with process_one_read's decisions.
+CRAMREC_HD inline void mate_replay(const uint32_t *members, uint32_t k, const Core *core, const int64_t *aend, uint8_t *cf, int32_t *nf)
+{
+    if (k < 2) return;
+    uint32_t pi = members[0];
+    MateRec p = mate_detached(core[pi], aend[pi]);
+    uint32_t r12 = ((core[pi].flag & 0x40) ? 1u : 0u) | ((core[pi].flag & 0x80) ? 2u : 0u);
+    for (uint32_t j = 1; j < k; j++) {
+        const uint32_t g = members[j];
+        const Core &b = core[g];
+        const int64_t apos = b.pos + 1;
+        const int64_t aleft = apos < p.apos ? apos : p.apos, aright = aend[g] > p.aend ? aend[g] : p.aend;
+        const int64_t sign = apos < p.apos ? 1 : apos > p.apos ? -1 : (b.flag & 0x40) ? 1 : -1;
+        const int64_t span = aright - aleft + 1;
+        const bool detach =
+            ((r12 & 1) && (b.flag & 0x40)) || ((r12 & 2) && (b.flag & 0x80)) ||                 // a repeated READ1 / READ2
+            (b.mpos + 1 > 0 ? b.mpos + 1 : 0) != p.apos ||
+            ((b.flag & 8) != 0) != ((p.flags & 4) != 0) || ((b.flag & 0x20) != 0) != ((p.flags & 0x10) != 0) ||
+            p.ref_id != b.tid || p.mate_pos != apos ||
+            ((p.flags & 8) != 0) != ((p.mate_flags & 2) != 0) || ((p.flags & 0x20) != 0) != ((p.mate_flags & 1) != 0) ||
+            ((b.flag | p.flags) & 0x800) ||                                                     // supplementary
+            b.isize == 0 || b.isize != sign * span || p.tlen == 0 || p.tlen != -sign * span;
+        if (detach) continue;                                                                   // cf[g] stays DETACHED, the entry stays at p
+        MateRec cr;
+        cr.apos = apos; cr.aend = aend[g]; cr.ref_id = b.tid; cr.flags = b.flag;
+        cr.mate_pos = p.apos;
+        cr.tlen = sign * span;
+        cr.mate_flags = ((p.flags & 8) ? 2u : 0u) | ((p.flags & 0x20) ? 1u : 0u);
+        cf[g] = 0;
+        cf[pi] = MATE_DOWNSTREAM;
+        nf[pi] = (int32_t)(g - pi - 1);
+        r12 |= ((b.flag & 0x40) ? 1u : 0u) | ((b.flag & 0x80) ? 2u : 0u);
+        p = cr; pi = g;
+    }
 }
 
 }  // namespace cramenc

@@ -37,6 +37,15 @@ using namespace cramrec;
 #ifdef HGPU_HOSTSIM
 #define hgpu_cram_records_free hostsim_cram_records_free
 extern "C" void hgpu_cram_records_free(hgpu_cram_records *r);
+// test hook: every record's cram_flags and mate_line as the record loop read them (before cram_decode_slice_xref
+// closes the mate chains), of the last decode; -1 / -1 for records of a slice that failed
+static std::vector<int32_t> g_rec_cram_flags, g_rec_mate_line;
+extern "C" uint64_t hostsim_cram_record_mates(int32_t *cram_flags, int32_t *mate_line, uint64_t cap)
+{
+    const uint64_t n = g_rec_cram_flags.size();
+    for (uint64_t i = 0; i < n && i < cap; i++) { cram_flags[i] = g_rec_cram_flags[i]; mate_line[i] = g_rec_mate_line[i]; }
+    return n;
+}
 #endif
 static_assert(sizeof(BamCore) == 48 && sizeof(hgpu_bam1_core) == 48, "bam1_core_t mirror");
 
@@ -585,6 +594,10 @@ CRAMREC_HD void slice_body(const Args &A, uint32_t si, uint32_t lane, uint32_t n
     if (rc == ERR_NONE) rc = S.req == SAM_ALL ? D.template decode_slice<false>(S, recs, A.nrg, A.unknown_rg)
                                               : D.template decode_slice<true>(S, recs, A.nrg, A.unknown_rg);
     W::sync();
+#ifdef HGPU_HOSTSIM
+    if (rc == ERR_NONE)
+        for (int32_t r = 0; r < S.n_records; r++) { g_rec_cram_flags[S.rec0 + r] = recs[r].cram_flags; g_rec_mate_line[S.rec0 + r] = recs[r].mate_line; }
+#endif
     if (rc == ERR_NONE && slice_xref(recs, S.n_records, S.req)) rc = ERR_DECODE;      // every lane runs it on the same data, same stores
     W::sync();
     // sizes: lanes take records
@@ -650,6 +663,9 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
                 int32_t req, hgpu_cram_records *out, hgpu_cram_records_dev *dev = nullptr)
 {
     if (dev) memset(dev, 0, sizeof *dev);
+#ifdef HGPU_HOSTSIM
+    g_rec_cram_flags.clear(); g_rec_mate_line.clear();
+#endif
     if (subset_mode(req) && !(req & SAM_AUX)) decode_md = 0;            // cram_decode.c:605-607
     // req == 0 reads every series like SAM_ALL, but cram_decode_slice_xref and cram_to_bam test the mask itself
     if (!file || !blocks || !udata || !udata_off || !out) { hgpu_set_error("cram records: null argument"); return HGPU_ERR_ARG; }
@@ -867,6 +883,7 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
     std::vector<int32_t> sstat(ns);
 #ifdef HGPU_HOSTSIM
     memset(L.at(s_cur), 0, ext.size() * 4);
+    g_rec_cram_flags.assign(n_records, -1); g_rec_mate_line.assign(n_records, -1);
     for (uint32_t s = 0; s < ns; s++) slice_body<HostW>(A, s, 0, 1);
     memcpy(sbytes.data(), A.slice_bytes, (size_t)ns * 8);
     memcpy(sstat.data(), A.slice_status, (size_t)ns * 4);

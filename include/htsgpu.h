@@ -480,19 +480,37 @@ typedef struct hgpu_cram_refs { const uint8_t *bases; const uint64_t *off; int32
  * cram_encode_slice cram/cram_encode.c:1950-2420, process_one_read :3490-4010, cram_encode_compression_header :380-1030,
  * container and file framing cram_io.c:3958-4100, :4694, :4889, :5512).  core / data / data_off: n records in
  * hgpu_bam_unpack_dev's layout (host arrays); header_text: the SAM header.  One slice of records_per_slice records
- * (0 = 10 000) per container.  On the device: per-record byte counts for each of the 31 series, a scan per (slice,
+ * (0 = 10 000) per container.  On the device: per-record byte counts for each series, a scan per (slice,
  * series), the series bytes; then every series block through the method trial of hgpu_cram_compress_blocks_host (rANS
  * Nx16 family for minor_version 1, rANS 4x8 for 0) and read names through the tok3 encoder (3.1), framed with CRC-32.
  * refs (may be NULL): with the reference sequence of every mapped record supplied, match operations are coded against
  * it — equal bases leave nothing, a differing base is a substitution feature — and the file needs that reference to
  * decode (RR = 1), as the reference's writer does; otherwise bases are explicit and the file decodes without one
- * (RR = 0).  Every mate is written detached, slices are multi-reference.  What the reference's reader returns for the
+ * (RR = 0).  Every mate is written detached (see hgpu_cram_encode_records_opts_host for mate attachment), slices are
+ * multi-reference.  What the reference's reader returns for the
  * file is the input records, except what CRAM cannot hold ('=' / 'X' CIGAR ops come back as 'M', MAPQ of unmapped reads
  * as 0, RNEXT of unpaired reads as '*').  HGPU_CRAM_UNSUPPORTED: a mapped read at position 0 or a zero-length CIGAR op
  * (left to the host library).  *out_file is malloc'd. */
 int hgpu_cram_encode_records_host(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, const hgpu_bam1_core *core,
         const uint8_t *data, const uint64_t *data_off, uint64_t n, const hgpu_cram_refs *refs, uint32_t records_per_slice,
         int minor_version, uint8_t **out_file, uint64_t *out_len);
+
+/* Writer options of hgpu_cram_encode_records_opts_host (a bit mask; unknown bits are refused with HGPU_ERR_ARG).
+ * HGPU_CRAM_ENC_ATTACH_MATES: reads of one template that fall in the same slice are attached as the reference's
+ * process_one_read attaches them (cram/cram_encode.c:3799-4012, CRAM 3.x, default options): when their mate fields
+ * can be rebuilt exactly, the earlier read gets CRAM_FLAG_MATE_DOWNSTREAM and an NF distance, neither stores MF / NS /
+ * NP / TS, and the reader rebuilds them.  Records that do not qualify stay detached.  Decided on the device by a
+ * pairing pass (a name table per slice, one thread per name group) before the count pass. */
+#define HGPU_CRAM_ENC_ATTACH_MATES 0x1u
+
+/* hgpu_cram_encode_records_host with writer options.  enc_flags = 0 gives the same bytes as
+ * hgpu_cram_encode_records_host (every mate detached, no NF series in the compression header). */
+int hgpu_cram_encode_records_opts_host(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, const hgpu_bam1_core *core,
+        const uint8_t *data, const uint64_t *data_off, uint64_t n, const hgpu_cram_refs *refs, uint32_t records_per_slice,
+        int minor_version, uint32_t enc_flags, uint8_t **out_file, uint64_t *out_len);
+/* measurement: device time (ms) of the last encode call's pairing kernels (0 without mate attachment) and of its
+ * count + scan + write kernels */
+void hgpu_cram_encode_last_ms(float *pair_ms, float *count_write_ms);
 
 /* CRAM 3.x record decode on the device — cram_decode_slice's record loop (cram/cram_decode.c:2340-3015), cram_decode_seq
  * (:1096-1917), cram_decode_aux (:2008-2137), cram_decode_slice_xref (:2140-2304) and cram_to_bam (:3100-3211) for every

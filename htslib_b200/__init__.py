@@ -343,6 +343,32 @@ class Context:
         lib().hgpu_bam_index_last_ms(ms)
         return ms[0], ms[1]
 
+    def cram_index(self, file_np):
+        """The .crai file of a whole CRAM 3.x image, as sam_index_build3 writes it (hgpu_cram_index_build_host): one gzip
+        member.  Raises HgpuError with .code and .bad (the slice, in file order, where the reference stops)."""
+        L = lib()
+        L.hgpu_cram_index_build_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64),
+                                                 C.POINTER(C.c_int64)]
+        L.hgpu_cram_index_build_host.restype = C.c_int
+        out, n, bad = C.c_void_p(), C.c_uint64(0), C.c_int64(-1)
+        rc = L.hgpu_cram_index_build_host(self.h, file_np.ctypes.data, file_np.size, C.byref(out), C.byref(n), C.byref(bad))
+        if rc != HGPU_OK:
+            e = HgpuError("cram_index failed: rc=%d bad=%d (%s)" % (rc, bad.value, last_error()))
+            e.code, e.bad = rc, bad.value
+            raise e
+        try:
+            return C.string_at(out, n.value)
+        finally:
+            libc = C.CDLL(None)
+            libc.free.argtypes = [C.c_void_p]
+            libc.free(out)
+
+    def cram_index_last_ms(self):
+        """(device ms of the slice decode and runs kernels, ms of the rest of the call) of the last cram_index call."""
+        ms = (C.c_float * 2)()
+        lib().hgpu_cram_index_last_ms(ms)
+        return ms[0], ms[1]
+
     def rans_nx16_decode_host(self, in_np, in_off, in_len, out_np, out_off, out_len):
         import numpy as np
         n = len(in_len)

@@ -1441,9 +1441,10 @@ __device__ __forceinline__ uint64_t token_bits_dyn(const DeflateDyn &d, uint32_t
 
 __device__ __forceinline__ uint32_t ld4(const uint8_t *p) { return p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
 
-// Returns the BGZF block length written to out (<= 65536), 0 on failure.
+// Returns the BGZF block length written to out (<= 65536), 0 on failure.  body_bits: bits of the deflate block that starts at
+// out[18] (its last byte is zero past them).
 __device__ uint32_t deflate_block_warp(DeflateSmem &s, const uint32_t (*crc_tab)[256], const uint8_t *in, uint32_t n,
-                                       int level, uint8_t *out, uint32_t *toks)
+                                       int level, uint8_t *out, uint32_t *toks, uint32_t &body_bits)
 {
     const uint32_t lane = hgpu_lane();
     if (n > 65280u) return 0;
@@ -1650,6 +1651,7 @@ __device__ uint32_t deflate_block_warp(DeflateSmem &s, const uint32_t (*crc_tab)
             }
             bitpos += eob_n;
             dlen = (uint32_t)((bitpos + 7) / 8) - 18;
+            body_bits = (uint32_t)(bitpos - 18 * 8);
             if (dlen >= n + 5) overflow = true;                    // stored would be smaller
         }
         __syncwarp();
@@ -1658,6 +1660,7 @@ __device__ uint32_t deflate_block_warp(DeflateSmem &s, const uint32_t (*crc_tab)
     }
     if (stored) {
         dlen = n + 5;
+        body_bits = 8 * dlen;
         __syncwarp();
         if (lane == 0) {
             out[18] = 1;                                            // BFINAL=1, BTYPE=00
@@ -1684,7 +1687,7 @@ __global__ void __launch_bounds__(128)
 bgzf_deflate_kernel(const uint8_t *__restrict__ in, const uint64_t *__restrict__ in_off,
                     const uint32_t *__restrict__ in_len, uint32_t n, int level, uint8_t *out,
                     const uint64_t *__restrict__ out_off, uint32_t *out_len, int32_t *status,
-                    uint32_t *toks_all, uint32_t *counter)
+                    uint32_t *body_bits, uint32_t *toks_all, uint32_t *counter)
 {
     __shared__ DeflateSmem smem_all[4];
     __shared__ uint32_t crc_tab[4][256];
@@ -1697,9 +1700,13 @@ bgzf_deflate_kernel(const uint8_t *__restrict__ in, const uint64_t *__restrict__
         if (hgpu_lane() == 0) job = atomicAdd(counter, 1u);
         job = __shfl_sync(0xffffffffu, job, 0);
         if (job >= n) break;
-        uint32_t got = deflate_block_warp(smem_all[w], crc_tab, in + in_off[job], in_len[job], level, out + out_off[job], toks);
+        uint32_t bits = 0;
+        uint32_t got = deflate_block_warp(smem_all[w], crc_tab, in + in_off[job], in_len[job], level, out + out_off[job], toks, bits);
         __syncwarp();
-        if (hgpu_lane() == 0) { out_len[job] = got; status[job] = got ? HGPU_OK : HGPU_BGZF_ERR_ZLIB; }
+        if (hgpu_lane() == 0) {
+            out_len[job] = got; status[job] = got ? HGPU_OK : HGPU_BGZF_ERR_ZLIB;
+            if (body_bits) body_bits[job] = bits;
+        }
     }
 }
 
@@ -1815,15 +1822,12 @@ int hgpu_launch_crc32_batch(hgpu_ctx *ctx, const uint8_t *d_buf, const uint64_t 
     return hgpu_check(cudaGetLastError(), "crc batch launch");
 }
 
-// Batch BGZF compress, device pointers.  Every out slot must be 65536 bytes and 4-byte aligned.
-extern "C" int hgpu_bgzf_compress_batch_dev(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off,
-        const uint32_t *d_in_len, uint32_t n, int level, uint8_t *d_out, const uint64_t *d_out_off,
-        uint32_t *d_out_len, int32_t *d_status, void *stream)
+int hgpu_launch_bgzf_deflate(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off, const uint32_t *d_in_len, uint32_t n,
+                             int level, uint8_t *d_out, const uint64_t *d_out_off, uint32_t *d_out_len, int32_t *d_status,
+                             uint32_t *d_body_bits, cudaStream_t st)
 {
-    if (!ctx) { hgpu_set_error("null context"); return HGPU_ERR_ARG; }
     if (n == 0) return HGPU_OK;
     if (level < 0) level = 6;                           // Z_DEFAULT_COMPRESSION, as zlib's deflateInit2 reads it
-    cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
     int rc = ensure_crc_tables(ctx, st);
     if (rc) return rc;
     int per_sm = 0;
@@ -1837,7 +1841,17 @@ extern "C" int hgpu_bgzf_compress_batch_dev(hgpu_ctx *ctx, const uint8_t *d_in, 
     uint32_t *counter = hgpu_take_counter(ctx, st);
     if (!counter) return HGPU_ERR_CUDA;
     bgzf_deflate_kernel<<<grid, 128, 0, st>>>(d_in, d_in_off, d_in_len, n, level, d_out, d_out_off, d_out_len, d_status,
-                                              reinterpret_cast<uint32_t *>(ctx->d_mrec), counter);
+                                              d_body_bits, reinterpret_cast<uint32_t *>(ctx->d_mrec), counter);
     hgpu_count_launch();
     return hgpu_check(cudaGetLastError(), "deflate launch");
+}
+
+// Batch BGZF compress, device pointers.  Every out slot must be 65536 bytes and 4-byte aligned.
+extern "C" int hgpu_bgzf_compress_batch_dev(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off,
+        const uint32_t *d_in_len, uint32_t n, int level, uint8_t *d_out, const uint64_t *d_out_off,
+        uint32_t *d_out_len, int32_t *d_status, void *stream)
+{
+    if (!ctx) { hgpu_set_error("null context"); return HGPU_ERR_ARG; }
+    return hgpu_launch_bgzf_deflate(ctx, d_in, d_in_off, d_in_len, n, level, d_out, d_out_off, d_out_len, d_status, nullptr,
+                                    stream ? (cudaStream_t)stream : ctx->stream);
 }

@@ -646,6 +646,11 @@ CRAMREC_HD void fill_body(const Args &A, uint64_t g)
 }
 
 #ifndef HGPU_HOSTSIM
+struct HgpuEvents {                                 // destroyed on every return path
+    cudaEvent_t e[2]; int n = 0;
+    bool make(int k) { for (; n < k; n++) if (cudaEventCreate(&e[n]) != cudaSuccess) return false; return true; }
+    ~HgpuEvents() { for (int k = 0; k < n; k++) cudaEventDestroy(e[k]); }
+};
 float g_last_ms[2] = {0, 0};                    // device time of the two kernels of the last call (bench.py reads it)
 __global__ void __launch_bounds__(32) cram_slice_decode_kernel(Args A)
 {
@@ -658,11 +663,22 @@ __global__ void __launch_bounds__(128) cram_bam_fill_kernel(Args A)
 }
 #endif
 
-int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n_blocks,
-                const uint8_t *udata, const uint64_t *udata_off, const hgpu_cram_refs *refs, const char *name_prefix, int decode_md,
-                int32_t req, hgpu_cram_records *out, hgpu_cram_records_dev *dev = nullptr)
+struct SliceRun {                                  // what decode_slices leaves for the pass after it
+    std::vector<uint8_t> image;                    // HGPU_HOSTSIM: the device image (A points into it)
+    Args A;
+    std::vector<int32_t> sstat;                    // per slice: the ERR_* of the slice decode
+    std::vector<uint64_t> sbytes;                  // per slice: bytes of its bam1_t data
+    uint64_t n_records = 0;
+    uint32_t ns = 0;
+    float ms = 0;                                  // device time of cram_slice_decode_kernel
+};
+
+// The framing, the tables, the upload and cram_slice_decode_kernel: every slice's Rec array in device memory (R.A.recs),
+// out->slice_status / slice_rec0 filled.  R.n_records == 0 when there is nothing to decode.
+int decode_slices(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n_blocks,
+                  const uint8_t *udata, const uint64_t *udata_off, const hgpu_cram_refs *refs, const char *name_prefix, int decode_md,
+                  int32_t req, hgpu_cram_records *out, SliceRun &R)
 {
-    if (dev) memset(dev, 0, sizeof *dev);
 #ifdef HGPU_HOSTSIM
     g_rec_cram_flags.clear(); g_rec_mate_line.clear();
 #endif
@@ -805,12 +821,7 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
     out->n_records = n_records; out->n_slices = ns;
     out->slice_status = (int32_t *)calloc(ns + 1, sizeof(int32_t));
     out->slice_rec0 = (uint64_t *)calloc((size_t)ns + 1, sizeof(uint64_t));
-    if (!dev) {
-        out->core = (hgpu_bam1_core *)calloc(n_records + 1, sizeof(hgpu_bam1_core));
-        out->data_off = (uint64_t *)calloc(n_records + 1, sizeof(uint64_t));
-        out->rec_status = (int32_t *)calloc(n_records + 1, sizeof(int32_t));
-    }
-    if (!out->slice_status || !out->slice_rec0 || (!dev && (!out->core || !out->data_off || !out->rec_status))) { hgpu_cram_records_free(out); hgpu_set_error("out of host memory"); return HGPU_ERR_NOMEM; }
+    if (!out->slice_status || !out->slice_rec0) { hgpu_cram_records_free(out); hgpu_set_error("out of host memory"); return HGPU_ERR_NOMEM; }
     for (uint32_t s = 0; s < ns; s++) out->slice_rec0[s] = slices[s].rec0;
     out->slice_rec0[ns] = n_records;
     if (ns == 0 || n_records == 0) return HGPU_OK;
@@ -829,8 +840,8 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
 
 #ifdef HGPU_HOSTSIM
     (void)ctx;
-    std::vector<uint8_t> image(L.total);
-    L.base = image.data();
+    R.image.assign(L.total, 0);
+    L.base = R.image.data();
 #define UP(seg, src, n) do { if (n) memcpy(L.at(seg), (src), (n)); } while (0)
 #else
     if (!ctx) { hgpu_set_error("null context"); return HGPU_ERR_ARG; }
@@ -859,7 +870,7 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
     UP(s_rgl, rg_len.data(), rg_len.size() * 4);
     UP(s_pre, name_prefix ? name_prefix : "", prefix_len);
 
-    Args A;
+    Args &A = R.A;
     memset(&A, 0, sizeof A);
     A.P.tables = L.at<Table>(s_tab); A.P.cpool = L.at<Codec>(s_cp);
     A.P.hpool = L.at<HuffCode>(s_hp); A.P.tagkeys = L.at<uint32_t>(s_tk);
@@ -879,8 +890,9 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
     A.core = L.at<BamCore>(s_core); A.data_off = L.at<uint64_t>(s_doff);
     A.rec_status = L.at<int32_t>(s_rst); A.n_records = n_records;
 
-    std::vector<uint64_t> sbytes(ns), sbase((size_t)ns + 1, 0);
-    std::vector<int32_t> sstat(ns);
+    std::vector<uint64_t> &sbytes = R.sbytes;
+    std::vector<int32_t> &sstat = R.sstat;
+    sbytes.assign(ns, 0); sstat.assign(ns, 0);
 #ifdef HGPU_HOSTSIM
     memset(L.at(s_cur), 0, ext.size() * 4);
     g_rec_cram_flags.assign(n_records, -1); g_rec_mate_line.assign(n_records, -1);
@@ -889,30 +901,52 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
     memcpy(sstat.data(), A.slice_status, (size_t)ns * 4);
 #else
     if (rc0 || (rc0 = hgpu_memset(L.at(s_cur), 0, ext.size() * 4 + 4, st))) return rc0;
-    struct Events {                                  // destroyed on every return path
-        cudaEvent_t e[4]; int n = 0;
-        bool make() { for (; n < 4; n++) if (cudaEventCreate(&e[n]) != cudaSuccess) return false; return true; }
-        ~Events() { for (int k = 0; k < n; k++) cudaEventDestroy(e[k]); }
-    } evs;
-    if (!evs.make()) return HGPU_ERR_CUDA;
-    cudaEvent_t *ev = evs.e;
-    cudaEventRecord(ev[0], st);
+    HgpuEvents evs;
+    if (!evs.make(2)) return HGPU_ERR_CUDA;
+    cudaEventRecord(evs.e[0], st);
     cram_slice_decode_kernel<<<ns, 32, 0, st>>>(A);
-    cudaEventRecord(ev[1], st);
+    cudaEventRecord(evs.e[1], st);
     hgpu_count_launch();
     if (hgpu_check(cudaGetLastError(), "cram slice decode launch")) return HGPU_ERR_CUDA;
     if (hgpu_d2h(sbytes.data(), A.slice_bytes, (size_t)ns * 8, st) || hgpu_d2h(sstat.data(), A.slice_status, (size_t)ns * 4, st)) return HGPU_ERR_CUDA;
     if (hgpu_check(cudaStreamSynchronize(st), "cram slice decode")) return HGPU_ERR_CUDA;
+    cudaEventElapsedTime(&R.ms, evs.e[0], evs.e[1]);
 #endif
-    for (uint32_t s = 0; s < ns; s++) { if (sstat[s] != 0) sbytes[s] = 0; sbase[s + 1] = sbase[s] + sbytes[s]; }
+    for (uint32_t s = 0; s < ns; s++) out->slice_status[s] = sstat[s] == ERR_SPACE ? HGPU_CRAM_ERR_SPACE : sstat[s] == ERR_NOREF ? HGPU_CRAM_ERR_NOREF : sstat[s];
+    R.ns = ns; R.n_records = n_records;
+#undef UP
+    return HGPU_OK;
+}
+
+// decode_slices, then cram_bam_fill_kernel: the records as bam1_t
+int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n_blocks,
+                const uint8_t *udata, const uint64_t *udata_off, const hgpu_cram_refs *refs, const char *name_prefix, int decode_md,
+                int32_t req, hgpu_cram_records *out, hgpu_cram_records_dev *dev = nullptr)
+{
+    if (dev) memset(dev, 0, sizeof *dev);
+    SliceRun R;
+    int rc = decode_slices(ctx, file, file_len, blocks, n_blocks, udata, udata_off, refs, name_prefix, decode_md, req, out, R);
+    if (rc) return rc;
+    const uint64_t n_records = out->n_records;
+    const uint32_t ns = (uint32_t)out->n_slices;
+    if (!dev) {
+        out->core = (hgpu_bam1_core *)calloc(n_records + 1, sizeof(hgpu_bam1_core));
+        out->data_off = (uint64_t *)calloc(n_records + 1, sizeof(uint64_t));
+        out->rec_status = (int32_t *)calloc(n_records + 1, sizeof(int32_t));
+        if (!out->core || !out->data_off || !out->rec_status) { hgpu_cram_records_free(out); hgpu_set_error("out of host memory"); return HGPU_ERR_NOMEM; }
+    }
+    if (ns == 0 || n_records == 0) return HGPU_OK;
+    Args &A = R.A;
+    std::vector<uint64_t> sbase((size_t)ns + 1, 0);
+    for (uint32_t s = 0; s < ns; s++) sbase[s + 1] = sbase[s] + (R.sstat[s] != 0 ? 0 : R.sbytes[s]);
     const uint64_t data_bytes = sbase[ns];
     out->data_bytes = data_bytes;
     if (!dev) out->data = (uint8_t *)malloc(data_bytes + 16);
     if (!dev && !out->data) { hgpu_cram_records_free(out); hgpu_set_error("out of host memory"); return HGPU_ERR_NOMEM; }
-    for (uint32_t s = 0; s < ns; s++) out->slice_status[s] = sstat[s] == ERR_SPACE ? HGPU_CRAM_ERR_SPACE : sstat[s] == ERR_NOREF ? HGPU_CRAM_ERR_NOREF : sstat[s];
 
 #ifdef HGPU_HOSTSIM
-    memcpy(L.at(s_sbase), sbase.data(), sbase.size() * 8);
+    (void)ctx;
+    memcpy(const_cast<uint64_t *>(A.slice_base), sbase.data(), sbase.size() * 8);
     std::vector<uint8_t> dbuf(data_bytes + 16);
     A.data = dbuf.data();
     for (uint64_t g = 0; g < n_records; g++) fill_body<HostW>(A, g);
@@ -925,10 +959,13 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
     int rc1 = hgpu_ensure_mrec(ctx, data_bytes + 256);            // (not d_bam: hgpu_sam_format_dev / hgpu_bam_pack_dev scan there)
     if (rc1) { hgpu_cram_records_free(out); return rc1; }
     A.data = ctx->d_mrec;
-    if (hgpu_h2d(L.at(s_sbase), sbase.data(), sbase.size() * 8, st)) return HGPU_ERR_CUDA;
-    cudaEventRecord(ev[2], st);
+    cudaStream_t st = ctx->stream;
+    HgpuEvents evs;
+    if (!evs.make(2)) return HGPU_ERR_CUDA;
+    if (hgpu_h2d(const_cast<uint64_t *>(A.slice_base), sbase.data(), sbase.size() * 8, st)) return HGPU_ERR_CUDA;
+    cudaEventRecord(evs.e[0], st);
     cram_bam_fill_kernel<<<(unsigned)((n_records + 3) / 4), 128, 0, st>>>(A);
-    cudaEventRecord(ev[3], st);
+    cudaEventRecord(evs.e[1], st);
     hgpu_count_launch();
     if (hgpu_check(cudaGetLastError(), "cram bam fill launch")) return HGPU_ERR_CUDA;
     if (dev) {
@@ -939,10 +976,9 @@ int decode_impl(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgp
             hgpu_d2h(out->rec_status, A.rec_status, n_records * 4, st) || hgpu_d2h(out->data, A.data, data_bytes, st)) return HGPU_ERR_CUDA;
     }
     if (hgpu_check(cudaStreamSynchronize(st), "cram bam fill")) return HGPU_ERR_CUDA;
-    cudaEventElapsedTime(&g_last_ms[0], ev[0], ev[1]);
-    cudaEventElapsedTime(&g_last_ms[1], ev[2], ev[3]);
+    g_last_ms[0] = R.ms;
+    cudaEventElapsedTime(&g_last_ms[1], evs.e[0], evs.e[1]);
 #endif
-#undef UP
     return HGPU_OK;
 }
 
@@ -978,6 +1014,33 @@ long required_blocks(const hgpu_cram_block *blocks, uint32_t n_blocks, const uin
 }
 
 }  // namespace
+
+namespace cramrec {
+int slice_records(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n_blocks,
+                  const uint8_t *udata, const uint64_t *udata_off, int32_t req, SliceRecs &out)
+{
+    hgpu_cram_records r;
+    memset(&r, 0, sizeof r);
+    SliceRun R;
+    const int rc = decode_slices(ctx, file, file_len, blocks, n_blocks, udata, udata_off, nullptr, nullptr, 0, req, &r, R);
+    if (rc == HGPU_OK) {
+        out.rec0.assign(r.slice_rec0, r.slice_rec0 + r.n_slices + 1);
+        out.status = R.sstat;
+        out.status.resize(r.n_slices, 0);
+        out.recs = R.A.recs;
+        out.image.swap(R.image);
+        out.ms = R.ms;
+    }
+    hgpu_cram_records_free(&r);
+    return rc;
+}
+
+bool compression_header_ok(const uint8_t *hdr, uint32_t len)
+{
+    Build B;
+    return build_table(B, hdr, len) == 0;
+}
+}  // namespace cramrec
 
 extern "C" void hgpu_cram_records_free(hgpu_cram_records *r)
 {

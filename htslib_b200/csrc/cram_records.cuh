@@ -1120,4 +1120,27 @@ CRAMREC_HD inline int bam_fill(const Rec *crecs, int32_t n, int32_t rec, const u
     return 0;
 }
 
+// ---- for passes of other files over the decoded records (cram_records.cu defines these; host code) ----
+}  // namespace cramrec
+#include <vector>
+struct hgpu_ctx;
+struct hgpu_cram_block;
+namespace cramrec {
+
+struct SliceRecs {                   // what cram_slice_decode_kernel left, for a pass of the caller's own
+    const Rec *recs = nullptr;       // every slice's records, slice after slice: device memory (host memory in the hostsim build),
+                                     // valid until the context stages its next call
+    std::vector<uint64_t> rec0;      // per slice: its first record; rec0[n_slices] = every record
+    std::vector<int32_t> status;     // per slice: 0 or the ERR_* of its decode
+    std::vector<uint8_t> image;      // hostsim build: the memory behind recs
+    float ms = 0;                    // device time of cram_slice_decode_kernel
+};
+
+// cram_slice_decode_kernel with the SAM_* mask req over the slices of a block list (as hgpu_cram_decode_records_fields_host
+// takes it), no reference and no bam1_t fill.  HGPU_OK or the error code of the records entry points.
+int slice_records(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len, const hgpu_cram_block *blocks, uint32_t n_blocks,
+                  const uint8_t *udata, const uint64_t *udata_off, int32_t req, SliceRecs &out);
+// cram_decode_compression_header accepts this uncompressed payload, as the record decoder reads it
+bool compression_header_ok(const uint8_t *hdr, uint32_t len);
+
 }  // namespace cramrec

@@ -138,6 +138,11 @@ int hgpu_launch_gzip_inflate(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t 
                              int32_t *d_status, cudaStream_t st);
 int hgpu_launch_crc32(hgpu_ctx *ctx, const uint8_t *d_buf, size_t len, uint32_t *d_partial,
                       uint32_t *h_result, uint32_t crc0, cudaStream_t st);
+// hgpu_bgzf_compress_batch_dev with, when d_body_bits is not null, the bit length of every job's deflate block (which starts
+// at byte 18 of its BGZF block) -- what a caller needs to splice the blocks into one deflate stream
+int hgpu_launch_bgzf_deflate(hgpu_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off, const uint32_t *d_in_len, uint32_t n,
+                             int level, uint8_t *d_out, const uint64_t *d_out_off, uint32_t *d_out_len, int32_t *d_status,
+                             uint32_t *d_body_bits, cudaStream_t st);
 
 // hgpu_bam_index_records_dev over a window of a longer record stream (bam_unpack.cu): a record that runs past len ends the
 // walk instead of breaking the chain, and *d_tail (device) receives where the walk stopped (len when whole records fill it)

@@ -473,6 +473,26 @@ int hgpu_bam_index_build_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_
  * window's compressed bytes are in HBM to the end of its index kernels, summed), ms2[1] host finishing (bins, file) */
 void hgpu_bam_index_last_ms(float *ms2);
 
+/* CRAI index of a whole CRAM 3.x image in host memory -- cram_index_build (cram/cram_index.c:779-848) as
+ * sam_index_build3(fn, fnidx, 0, 0) runs it.  *out (malloc'd, *out_len bytes) is the .crai: one gzip member, as
+ * bgzf_open(fn, "wg") writes it, whose inflated text equals the reference's byte for byte (the compressed bytes are this
+ * library's).  A slice with ref_seq_id != -2 gives its line from its header; a multi-reference slice is decoded on the device
+ * with the fields SAM_RNAME | SAM_POS | SAM_CIGAR and gives one line per run of records with equal ref_id.  No reference
+ * sequence is read.  Returns HGPU_OK, or, with *bad = the slice (in file order) where the reference stops, -1 for the file
+ * header:
+ *   HGPU_IDX_ERR_PUSH  a container starts before the one ahead of it on the same reference (the reference returns -2);
+ *   HGPU_IDX_ERR_READ  the reference returns -1: a compression header or slice that will not read (truncated, a CRC failure,
+ *                      malformed), a slice offset that is not its landmark, a container length that is not its blocks', a slice
+ *                      over INT_MAX bytes, a multi-reference slice that fails to decode or whose records go backwards on one
+ *                      reference (cram_index_slice's -2 reaches the caller as -1);
+ *   HGPU_ERR_ARG       not CRAM 3.x.
+ * A container header that will not read (truncated, CRC failure) ends the index there, as in the reference. */
+int  hgpu_cram_index_build_host(hgpu_ctx *ctx, const uint8_t *file, uint64_t file_len,
+                                uint8_t **out, uint64_t *out_len, int64_t *bad);
+/* milliseconds of the last hgpu_cram_index_build_host: ms2[0] device time (CUDA events over the slice decode and the runs
+ * kernels), ms2[1] the rest of the call (walk, block uncompress, deflate, copies) */
+void hgpu_cram_index_last_ms(float *ms2);
+
 /* the reference sequences of a file, for the CRAM record decoder and encoder: upper case, @SQ order, back to back */
 typedef struct hgpu_cram_refs { const uint8_t *bases; const uint64_t *off; int32_t n_ref; } hgpu_cram_refs;
 

@@ -21,8 +21,11 @@
 namespace {
 
 constexpr int LIT_ROOT = 9, DST_ROOT = 8;
-constexpr int LIT_TABLE = (1 << LIT_ROOT) + 856;    // zlib "enough 286 9 15" = 852 sub-table slots
-constexpr int DST_TABLE = (1 << DST_ROOT) + 512;    // 30 symbols / 8 root bits: < 4 groups x 128
+// Sub-table room.  A complete code of 286 symbols, at most 15 bits, with a 9-bit root needs at most 340 sub-table
+// entries (zlib's "enough 286 9 15" = 852 counts the 512 root entries too); 30 distance symbols with an 8-bit root
+// need at most 144 (400 in all).  test_gpu_bgzf_huffman builds both worst cases.
+constexpr int LIT_TABLE = (1 << LIT_ROOT) + 856;
+constexpr int DST_TABLE = (1 << DST_ROOT) + 512;
 constexpr int CL_TABLE = 128;
 
 // entry kinds: one bit each for literal / length / distance / end-of-block (so a symbol loop can test them without
@@ -702,6 +705,9 @@ __device__ int decode_body_uniform(InflateSmem &s, Bits &b, uint8_t *out, uint32
         uint32_t e = lookup<LIT_ROOT>(s.lit, b);
         uint32_t kind = (e >> 4) & 15;
         if (kind == K_LIT) {
+            // past the input bits_fill supplies zero bits: a truncated stream whose all-zeros code is a literal would
+            // otherwise fill the slot with it and come back ERR_SPACE instead of an inflate error
+            if (bits_overrun(b)) return HGPU_BGZF_ERR_ZLIB;
             if (o >= cap) return HGPU_BGZF_ERR_SPACE;
             if (lane == 0) out[o] = (uint8_t)(e >> 16);
             o++;

@@ -6,8 +6,9 @@
 // input; the bytes are this encoder's own where the reference's parameter search is not reproduced:
 //   * one parameter block, no selector (the reference may split READ1/READ2 or by average quality,
 //     fqz_qual_stats :392-672); qualities are stored in their original orientation (CRAM >= 3.1);
-//   * the strategy rows (strat_opts :195-202) and their size / alphabet adjustments (:805-833), the
-//     quality map for <= 8 symbols, fixed-length detection, the position and delta tables and the
+//   * the strategy rows (strat_opts :195-202), the context bits rows 0 and 1 set aside for a selector
+//     (:601-622, applied by the reference even where it then keeps no selector), the size / alphabet
+//     adjustments (:805-833), the quality map for <= 8 symbols, fixed-length detection, the position and delta tables and the
 //     duplicate-record flag (a record equal to the previous one costs one symbol) are the reference's.
 // Work split: the host reads each block once (histogram, lengths, duplicates) and writes the parameter
 // block (fqz_store_parameters :674-733, store_array :102-144); the device initialises the 65 536 models
@@ -246,7 +247,9 @@ static int hgpu_fqz_encode_batch_host_impl(hgpu_ctx *ctx, const uint8_t *in, con
     // ---- host: parameters of every stream (fqz_pick_parameters :736-924 without the selector search)
     std::vector<EncStream> streams(n);
     std::vector<EncParam> params(n);
-    uint64_t model_words = 0;
+    const uint64_t MODEL_BUDGET = 6ull << 30;
+    std::vector<uint32_t> wave_first(1, 0u);                              // first stream of every wave
+    uint64_t model_words = 0 /* largest wave */, wave_words = 0;
     const uint64_t in_end = hgpu_slots_end(in_off, in_len, n), out_end = hgpu_slots_end(out_off, out_cap, n),
                    rec_end = hgpu_slots_end(rec_off, nrec, n);
     for (uint32_t s = 0; s < n; s++) {
@@ -278,7 +281,12 @@ static int hgpu_fqz_encode_batch_host_impl(hgpu_ctx *ctx, const uint8_t *in, con
         for (uint32_t r = 1; r < nrec[s]; r++) if (L[r] != L[0]) { fixed_len = false; break; }
         int qbits = strat_opts[strat][0], qshift = strat_opts[strat][1], pbits = strat_opts[strat][2], pshift = strat_opts[strat][3],
             dbits = strat_opts[strat][4], dshift = strat_opts[strat][5];
-        const int qloc = strat_opts[strat][6], sloc = strat_opts[strat][7], ploc = strat_opts[strat][8], dloc = strat_opts[strat][9];
+        int qloc = strat_opts[strat][6], sloc = strat_opts[strat][7], ploc = strat_opts[strat][8], dloc = strat_opts[strat][9];
+        if (strat_opts[strat][11] == -1) {                                 // qa -1 frees context bits for a selector (:601-622),
+            if (pbits > 0 && dbits > 0) { sloc = dloc - 1; pbits--; dbits--; dloc++; }   // whether or not one is kept
+            else if (dbits >= 2) { sloc = dloc; dbits -= 2; dloc += 2; }
+            else if (qbits >= 2) { qbits -= 2; ploc -= 2; sloc = 16 - 2 - strat_opts[strat][10]; if (qbits == 6 && qshift == 5) qbits--; }
+        }
         const bool store_qmap = nsym <= 8 && nsym * 2 < max_sym;
         if (pshift < 0) { double v = log((double)L[0] / (1 << pbits)) / log(2.0) + .5; pshift = v > 0 ? (int)v : 0; }
         if (nsym <= 4) { qshift = 2; if (size < 5000000) { pbits = 2; pshift = 5; } }
@@ -320,10 +328,16 @@ static int hgpu_fqz_encode_batch_host_impl(hgpu_ctx *ctx, const uint8_t *in, con
         P.fixed_len = fixed_len; P.do_dedup = do_dedup; P.nsym = sym_max + 1;
         for (int i = 0; i < 1024; i++) P.ptab[i] = ptab[i] << ploc;
         for (int i = 0; i < 256; i++) P.dtab[i] = dtab[i] << dloc;
-        S.model_off = model_words;
-        model_words += (uint64_t)CTX_SIZE * (P.nsym + 4) + 4 * 260 + 6 + 16;
+        // model arenas per WAVE, as the decoder hands them out (fqzcomp.cu): a wave's arenas fit MODEL_BUDGET (one
+        // stream alone may exceed it) and the next wave reuses the memory
+        const uint64_t words = (uint64_t)CTX_SIZE * (P.nsym + 4) + 4 * 260 + 6 + 16;
+        if (wave_words && (wave_words + words) * 4 > MODEL_BUDGET) { wave_first.push_back(s); wave_words = 0; }
+        S.model_off = wave_words;
+        wave_words += words;
+        if (wave_words > model_words) model_words = wave_words;
         S.host_status = HGPU_OK;
     }
+    wave_first.push_back(n);
 
     StageLayout L;
     const auto s_in = L.seg(in_end + 8), s_out = L.seg(out_end + 8), s_rec = L.seg(rec_end * 4 + 8), s_streams = L.seg((size_t)n * sizeof(EncStream)),
@@ -337,16 +351,20 @@ static int hgpu_fqz_encode_batch_host_impl(hgpu_ctx *ctx, const uint8_t *in, con
     if (hgpu_h2d(L.at(s_in), in, in_end, st) || hgpu_h2d(L.at(s_out), out, out_end, st) /* the headers */ ||
         hgpu_h2d(L.at(s_rec), rec_len, rec_end * 4, st) || hgpu_h2d(L.at(s_streams), streams.data(), (size_t)n * sizeof(EncStream), st) ||
         hgpu_h2d(L.at(s_params), params.data(), (size_t)n * sizeof(EncParam), st)) return HGPU_ERR_CUDA;
-    for (uint32_t first = 0; first < n; first += 65535u) {
-        const uint32_t cnt = n - first < 65535u ? n - first : 65535u;
-        fqz_enc_init_models_kernel<<<dim3(64, cnt), 256, 0, st>>>(d_streams + first, d_params + first, L.at<uint32_t>(s_models));
-        if (hgpu_check(cudaGetLastError(), "fqz_enc_init_models_kernel")) return HGPU_ERR_CUDA;
+    for (size_t w = 0; w + 1 < wave_first.size(); w++) {                 // waves run back to back on one stream: the arena is reused
+        const uint32_t w0 = wave_first[w], wend = wave_first[w + 1];
+        if (w0 == wend) continue;
+        for (uint32_t first = w0; first < wend; first += 65535u) {       // gridDim.y limit
+            const uint32_t cnt = wend - first < 65535u ? wend - first : 65535u;
+            fqz_enc_init_models_kernel<<<dim3(64, cnt), 256, 0, st>>>(d_streams + first, d_params + first, L.at<uint32_t>(s_models));
+            if (hgpu_check(cudaGetLastError(), "fqz_enc_init_models_kernel")) return HGPU_ERR_CUDA;
+            hgpu_count_launch();
+        }
+        fqz_encode_kernel<<<(wend - w0 + 31) / 32, 32, 0, st>>>(d_streams, d_params, w0, wend, L.at(s_in), L.at<uint32_t>(s_rec),
+                                                                L.at<uint32_t>(s_models), L.at(s_out), L.at<uint32_t>(s_olen), L.at<int32_t>(s_st));
+        if (hgpu_check(cudaGetLastError(), "fqz_encode_kernel")) return HGPU_ERR_CUDA;
         hgpu_count_launch();
     }
-    fqz_encode_kernel<<<(n + 31) / 32, 32, 0, st>>>(d_streams, d_params, 0, n, L.at(s_in), L.at<uint32_t>(s_rec), L.at<uint32_t>(s_models),
-                                                   L.at(s_out), L.at<uint32_t>(s_olen), L.at<int32_t>(s_st));
-    if (hgpu_check(cudaGetLastError(), "fqz_encode_kernel")) return HGPU_ERR_CUDA;
-    hgpu_count_launch();
     if (hgpu_d2h(out_len, L.at(s_olen), (size_t)n * 4, st) || hgpu_d2h(status, L.at(s_st), (size_t)n * 4, st) ||
         hgpu_d2h(out, L.at(s_out), out_end, st)) return HGPU_ERR_CUDA;
     if (hgpu_check(cudaStreamSynchronize(st), "sync")) return HGPU_ERR_CUDA;

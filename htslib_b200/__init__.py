@@ -547,6 +547,7 @@ def cram_decode_records(ctx, file_np, blocks, udata, udata_off, fasta=None, pref
 
 
 CRAM_ENC_ATTACH_MATES = 0x1          # HGPU_CRAM_ENC_ATTACH_MATES
+CRAM_ENC_TAG_BLOCKS = 0x2            # HGPU_CRAM_ENC_TAG_BLOCKS
 
 
 def cram_encode_records(ctx, header_text, core, data, data_off, n, fasta=None, records_per_slice=0, minor_version=1, enc_flags=0):
@@ -571,6 +572,13 @@ def cram_encode_last_ms():
     a, b = C.c_float(0), C.c_float(0)
     lib().hgpu_cram_encode_last_ms(C.byref(a), C.byref(b))
     return a.value, b.value
+
+
+def cram_encode_tags_last_ms():
+    """Device ms of the tag pass of the last cram_encode_records call (0 when it did not run)."""
+    a = C.c_float(0)
+    lib().hgpu_cram_encode_tags_last_ms(C.byref(a))
+    return a.value
 
 
 # CRAM_OPT_REQUIRED_FIELDS bits (htslib's SAM_*, hts.h:279-291; HGPU_SAM_* in htsgpu.h)

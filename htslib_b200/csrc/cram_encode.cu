@@ -27,11 +27,14 @@ struct hgpu_ctx;
 #include "cram_encode.cuh"
 #include "stage_layout.h"
 #include <map>
+#include <set>
 #include <string>
 #include <vector>
 #ifdef HGPU_HOSTSIM
 static std::vector<uint8_t> g_mate_cf;             // the pairing pass's decisions of the last call with mate attachment
 static std::vector<int32_t> g_mate_nf;
+static std::vector<uint8_t> g_tag_drop;            // the tag pass's drop bits and the RG series values of the last call with tag blocks
+static std::vector<int32_t> g_tag_rg;
 #endif
 #include <stdlib.h>
 #include <string.h>
@@ -41,6 +44,9 @@ using namespace cramenc;
 namespace {
 
 static_assert(sizeof(Core) == 48 && sizeof(hgpu_bam1_core) == 48, "bam1_core_t mirror");
+// tag keys (one series each) a call with tag blocks may hold: bounds the per-(slice, series) count array at
+// (S_COUNT + 256) * 4 bytes per record
+constexpr uint32_t k_max_tag_keys = 256;
 
 uint32_t host_crc32(const uint8_t *p, size_t n, uint32_t crc = 0)         // container headers (a few dozen bytes each)
 {
@@ -91,7 +97,8 @@ void enc_byte_array_len(Buf &o, int len_id, int val_id)
 }
 
 // cram_encode_compression_header :380-1030 for this writer's fixed layout
-void compression_header(Buf &o, const std::vector<std::string> &tag_lines, const std::vector<uint32_t> &tag_keys, bool ref_required, bool attach)
+void compression_header(Buf &o, const std::vector<std::string> &tag_lines, const std::vector<uint32_t> &tag_keys, bool ref_required, bool attach,
+                        bool tag_blocks)
 {
     Buf pm;                                                                // preservation map
     pm.itf8(5);
@@ -118,7 +125,20 @@ void compression_header(Buf &o, const std::vector<std::string> &tag_lines, const
     o.itf8((int32_t)rm.v.size()); o.bytes(rm.v.data(), rm.v.size());
     Buf tm;                                                                // tag encoding map
     tm.itf8((int32_t)tag_keys.size());
-    for (uint32_t k : tag_keys) { tm.itf8((int32_t)k); enc_byte_array_len(tm, S_TAG_LEN + 1, S_TAG_VAL + 1); }
+    for (uint32_t k : tag_keys) {
+        tm.itf8((int32_t)k);
+        if (!tag_blocks) { enc_byte_array_len(tm, S_TAG_LEN + 1, S_TAG_VAL + 1); continue; }
+        // the codec cram_encode_aux gives each type (:2931-3033, CRAM 3.x); the key is the block's content id
+        const uint8_t t = (uint8_t)k;
+        if (t == 'Z' || t == 'H') { Buf a; a.u8('\t'); a.itf8((int32_t)k); tm.itf8(5); tm.itf8((int32_t)a.v.size()); tm.bytes(a.v.data(), a.v.size()); }
+        else if (t == 'B') enc_byte_array_len(tm, (int)k, (int)k);
+        else {                                                             // HUFFMAN with the value size as its only symbol
+            Buf h; h.itf8(1); h.itf8(t == 's' || t == 'S' ? 2 : t == 'i' || t == 'I' || t == 'f' ? 4 : 1); h.itf8(1); h.itf8(0);
+            Buf a; a.itf8(3); a.itf8((int32_t)h.v.size()); a.bytes(h.v.data(), h.v.size());
+            enc_external(a, (int)k);
+            tm.itf8(4); tm.itf8((int32_t)a.v.size()); tm.bytes(a.v.data(), a.v.size());
+        }
+    }
     o.itf8((int32_t)tm.v.size()); o.bytes(tm.v.data(), tm.v.size());
 }
 
@@ -133,7 +153,28 @@ struct EArgs {
     int32_t *status;                        // per record
     const uint8_t *mate_cf;                 // per record: the pairing pass's CF bits (nullptr: every record detached)
     const int32_t *mate_nf;                 // per record: NF of MATE_DOWNSTREAM records
+    uint32_t R;                             // series per slice: S_COUNT, + one per tag key with tag blocks
+    const uint32_t *tkeys; uint32_t ntk;    // tag blocks: the call's tag keys, sorted (stream S_COUNT + k); nullptr: shared streams
+    const uint8_t *tdrop;                   // per record: the tag pass's TAG_DROP_* bits (nullptr: nothing dropped)
+    const int32_t *rg;                      // per record: RG series value, >= 0 when its RG:Z leaves the tag line
 };
+
+CRAMREC_HD inline TagRec tag_rec(const EArgs &A, uint64_t g)
+{
+    TagRec T{A.tkeys, A.ntk, 0u, -1};
+    if (A.tkeys) { T.drop = A.tdrop ? A.tdrop[g] : 0u; T.rg = A.rg[g]; }
+    return T;
+}
+
+// the tag pass: TAG_DROP_* bits of every record, against its own reference sequence (reference-coded shape only)
+struct TArgs { const Core *core; const uint8_t *data; const uint64_t *data_off; const uint8_t *ref_bases; const uint64_t *ref_off; int32_t n_ref; uint64_t n; uint8_t *drop; };
+CRAMREC_HD inline void tags_body(const TArgs &A, uint64_t g)
+{
+    const int32_t t = A.core[g].tid;
+    const bool has = t >= 0 && t < A.n_ref;
+    A.drop[g] = (uint8_t)tag_rules(A.core[g], A.data + A.data_off[g], (uint32_t)(A.data_off[g + 1] - A.data_off[g]),
+                                   has ? A.ref_bases + A.ref_off[t] : nullptr, has ? (int64_t)(A.ref_off[t + 1] - A.ref_off[t]) : 0);
+}
 
 // the pairing pass: key (hash, aend) -> group (open-addressing name table per slice) -> scan of the group sizes ->
 // member lists -> resolve (one thread per group replays process_one_read's rule in record order)
@@ -254,12 +295,13 @@ CRAMREC_HD inline void count_body(const EArgs &A, uint64_t g)
     uint32_t n[S_COUNT];
     for (int s = 0; s < S_COUNT; s++) n[s] = 0;
     Emit<false> E{n, nullptr};
+    if (A.tkeys) { E.x = A.cnt + ((size_t)sl * A.R + S_COUNT) * A.rps + r; E.xs = A.rps; }       // zeroed before the count pass
     const uint8_t *ref = nullptr; int64_t rl = 0;
     if (A.ref_bases && A.core[g].tid >= 0 && A.core[g].tid < A.n_ref) { ref = A.ref_bases + A.ref_off[A.core[g].tid]; rl = (int64_t)(A.ref_off[A.core[g].tid + 1] - A.ref_off[A.core[g].tid]); }
     const int rc = walk<false>(A.core[g], A.data + A.data_off[g], (uint32_t)(A.data_off[g + 1] - A.data_off[g]), A.tl[g], ref, rl,
-                               A.mate_cf ? A.mate_cf[g] : MATE_DETACHED, A.mate_nf ? A.mate_nf[g] : 0, E);
+                               A.mate_cf ? A.mate_cf[g] : MATE_DETACHED, A.mate_nf ? A.mate_nf[g] : 0, tag_rec(A, g), E);
     A.status[g] = rc;
-    for (int s = 0; s < S_COUNT; s++) A.cnt[((size_t)sl * S_COUNT + s) * A.rps + r] = rc == ENC_OK ? n[s] : 0;
+    for (int s = 0; s < S_COUNT; s++) A.cnt[((size_t)sl * A.R + s) * A.rps + r] = rc == ENC_OK ? n[s] : 0;
 }
 
 CRAMREC_HD inline void write_body(const EArgs &A, uint64_t g)
@@ -268,12 +310,13 @@ CRAMREC_HD inline void write_body(const EArgs &A, uint64_t g)
     const uint32_t sl = (uint32_t)(g / A.rps), r = (uint32_t)(g % A.rps);
     uint32_t n[S_COUNT];
     uint8_t *base[S_COUNT];
-    for (int s = 0; s < S_COUNT; s++) { n[s] = A.cnt[((size_t)sl * S_COUNT + s) * A.rps + r]; base[s] = A.arena + A.base[(size_t)sl * S_COUNT + s]; }
+    for (int s = 0; s < S_COUNT; s++) { n[s] = A.cnt[((size_t)sl * A.R + s) * A.rps + r]; base[s] = A.arena + A.base[(size_t)sl * A.R + s]; }
     Emit<true> E{n, base};
+    if (A.tkeys) { E.x = A.cnt + ((size_t)sl * A.R + S_COUNT) * A.rps + r; E.xs = A.rps; E.xarena = A.arena; E.xbase = A.base + (size_t)sl * A.R + S_COUNT; }
     const uint8_t *ref = nullptr; int64_t rl = 0;
     if (A.ref_bases && A.core[g].tid >= 0 && A.core[g].tid < A.n_ref) { ref = A.ref_bases + A.ref_off[A.core[g].tid]; rl = (int64_t)(A.ref_off[A.core[g].tid + 1] - A.ref_off[A.core[g].tid]); }
     walk<true>(A.core[g], A.data + A.data_off[g], (uint32_t)(A.data_off[g + 1] - A.data_off[g]), A.tl[g], ref, rl,
-               A.mate_cf ? A.mate_cf[g] : MATE_DETACHED, A.mate_nf ? A.mate_nf[g] : 0, E);
+               A.mate_cf ? A.mate_cf[g] : MATE_DETACHED, A.mate_nf ? A.mate_nf[g] : 0, tag_rec(A, g), E);
 }
 
 #ifndef HGPU_HOSTSIM
@@ -287,7 +330,7 @@ __global__ void __launch_bounds__(128) cram_enc_scan_kernel(EArgs A, uint32_t ro
 {
     const uint32_t row = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (row >= rows) return;
-    const uint32_t sl = row / S_COUNT;
+    const uint32_t sl = row / A.R;
     const uint64_t first = (uint64_t)sl * A.rps;
     const uint32_t nr = (uint32_t)(A.n - first < A.rps ? A.n - first : A.rps);
     uint32_t *p = A.cnt + (size_t)row * A.rps;
@@ -307,7 +350,13 @@ __global__ void __launch_bounds__(128) cram_enc_write_kernel(EArgs A)
     if (g < A.n) write_body(A, g);
 }
 
-float g_enc_ms[2] = {0, 0};                    // device time of the last call: pairing kernels, count + scan + write kernels
+float g_enc_ms[3] = {0, 0, 0};                 // device time of the last call: pairing kernels, count + scan + write kernels, tag pass
+// one thread per record: the MD / NM decisions of tag_rules
+__global__ void __launch_bounds__(128) cram_enc_tags_kernel(TArgs A)
+{
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g < A.n) tags_body(A, g);
+}
 __global__ void __launch_bounds__(128) cram_mate_key_kernel(PArgs A)
 {
     const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -350,9 +399,9 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
                 const uint64_t *data_off, uint64_t n, const hgpu_cram_refs *refs, uint32_t rps, int minor, uint32_t enc_flags,
                 uint8_t **out_file, uint64_t *out_len)
 {
-    const bool attach = (enc_flags & HGPU_CRAM_ENC_ATTACH_MATES) != 0;
+    const bool attach = (enc_flags & HGPU_CRAM_ENC_ATTACH_MATES) != 0, tb = (enc_flags & HGPU_CRAM_ENC_TAG_BLOCKS) != 0;
 #ifdef HGPU_HOSTSIM
-    g_mate_cf.clear(); g_mate_nf.clear();
+    g_mate_cf.clear(); g_mate_nf.clear(); g_tag_drop.clear(); g_tag_rg.clear();
 #endif
     // reference-based shape only when every mapped record's reference sequence was supplied (the reader will need them all)
     bool use_ref = refs && refs->bases && refs->off && refs->n_ref > 0;
@@ -366,39 +415,92 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
     *out_file = nullptr; *out_len = 0;
     if (rps == 0) rps = 10000;
     if (minor != 0 && minor != 1) { hgpu_set_error("cram encode: CRAM 3.0 or 3.1"); return HGPU_ERR_ARG; }
-    if (enc_flags & ~(uint32_t)HGPU_CRAM_ENC_ATTACH_MATES) { hgpu_set_error("cram encode: unknown flags 0x%x", enc_flags); return HGPU_ERR_ARG; }
+    if (enc_flags & ~(uint32_t)(HGPU_CRAM_ENC_ATTACH_MATES | HGPU_CRAM_ENC_TAG_BLOCKS)) { hgpu_set_error("cram encode: unknown flags 0x%x", enc_flags); return HGPU_ERR_ARG; }
     if (attach && rps > (1u << 29)) { hgpu_set_error("cram encode: records per slice above 2^29 with mate attachment"); return HGPU_ERR_ARG; }
     const uint32_t ns = (uint32_t)((n + rps - 1) / rps);
-    // ---- tag dictionary per slice (host: one walk over the aux field headers) ----
+    // aux fields of record g after SEQ / QUAL (nullptr when the record is too short: the count pass flags it)
+    auto aux_of = [&](uint64_t g) -> const uint8_t * {
+        const hgpu_bam1_core &c = core[g];
+        const uint64_t fixed = (uint64_t)c.l_qname + 4ull * c.n_cigar + ((uint64_t)(c.l_qseq < 0 ? 0 : c.l_qseq) + 1) / 2 + (uint64_t)(c.l_qseq < 0 ? 0 : c.l_qseq);
+        return fixed <= data_off[g + 1] - data_off[g] ? data + data_off[g] + fixed : nullptr;
+    };
+    // ---- tag blocks (host): the header's @RG IDs, each record's RG series value, the call's tag keys ----
+    std::vector<int32_t> rgv;
+    std::vector<uint32_t> tkeys;
+    if (tb) {
+        std::map<std::string, int32_t> rg_id;                              // sam_hrecs_find_rg: ID -> line index, the first line of an ID
+        for (uint32_t i = 0; i < header_len;) {
+            uint32_t e = i;
+            while (e < header_len && header_text[e] != '\n') e++;
+            if (e - i > 4 && !memcmp(header_text + i, "@RG\t", 4))
+                for (uint32_t f = i + 3; f < e; f++)
+                    if (header_text[f] == '\t' && f + 3 < e && !memcmp(header_text + f + 1, "ID:", 3)) {
+                        uint32_t v = f + 4, ve = v;
+                        while (ve < e && header_text[ve] != '\t' && header_text[ve] != '\r') ve++;
+                        const std::string id(header_text + v, ve - v);
+                        if (!rg_id.count(id)) { const int32_t k = (int32_t)rg_id.size(); rg_id[id] = k; }
+                        break;
+                    }
+            i = e + 1;
+        }
+        rgv.assign(n ? n : 1, -1);
+        std::set<uint32_t> ks;
+        for (uint64_t g = 0; g < n; g++) {
+            const uint8_t *p = aux_of(g), *end = data + data_off[g + 1];
+            int md = 0, nm = 0, rgz = 0;
+            for (; p && p < end;) {
+                uint32_t vlen = 0;
+                if (!aux_field(p, end, vlen)) break;                       // the count pass flags the record
+                md += p[0] == 'M' && p[1] == 'D'; nm += p[0] == 'N' && p[1] == 'M';
+                if (p[2] == 'd') { hgpu_set_error("cram encode: record %llu has an aux field of type 'd', which CRAM 3 tag blocks cannot hold", (unsigned long long)g); return HGPU_CRAM_UNSUPPORTED; }
+                if (p[0] == 'R' && p[1] == 'G' && p[2] == 'Z') {
+                    rgz++;
+                    auto it = rg_id.find(std::string((const char *)p + 3, vlen - 1));
+                    if (it != rg_id.end()) rgv[g] = it->second;
+                }
+                if (!(p[0] == 'R' && p[1] == 'G' && p[2] == 'Z' && rgv[g] >= 0)) ks.insert(aux_key(p));
+                p += 3 + vlen;
+            }
+            if (md > 1 || nm > 1 || rgz > 1) { hgpu_set_error("cram encode: record %llu repeats an MD, NM or RG tag", (unsigned long long)g); return HGPU_CRAM_UNSUPPORTED; }
+        }
+        if (ks.size() > k_max_tag_keys) { hgpu_set_error("cram encode: %zu distinct tag keys, above the %u tag blocks a call may hold", ks.size(), k_max_tag_keys); return HGPU_CRAM_UNSUPPORTED; }
+        tkeys.assign(ks.begin(), ks.end());
+    }
+    // ---- tag dictionary per slice (host: one walk over the aux field headers), without what the tag pass dropped ----
     std::vector<int32_t> tl(n ? n : 1, 0);
     std::vector<std::vector<std::string>> lines(ns);
     std::vector<std::vector<uint32_t>> keys(ns);
-    for (uint32_t sl = 0; sl < ns; sl++) {
-        std::map<std::string, int32_t> seen;
-        std::map<uint32_t, int> kseen;
-        const uint64_t a = (uint64_t)sl * rps, b = a + rps < n ? a + rps : n;
-        for (uint64_t g = a; g < b; g++) {
-            const hgpu_bam1_core &c = core[g];
-            const uint8_t *d = data + data_off[g], *end = data + data_off[g + 1];
-            const uint64_t fixed = (uint64_t)c.l_qname + 4ull * c.n_cigar + ((uint64_t)(c.l_qseq < 0 ? 0 : c.l_qseq) + 1) / 2 + (uint64_t)(c.l_qseq < 0 ? 0 : c.l_qseq);
-            std::string line;
-            if (fixed <= (uint64_t)(end - d)) {
-                for (const uint8_t *p = d + fixed; p < end;) {
-                    uint32_t vlen = 0;
-                    if (!aux_field(p, end, vlen)) break;                   // the count pass flags the record
-                    line.append((const char *)p, 3);
-                    const uint32_t key = (uint32_t)p[0] << 16 | (uint32_t)p[1] << 8 | p[2];
-                    if (!kseen.count(key)) { kseen[key] = 1; keys[sl].push_back(key); }
-                    p += 3 + vlen;
+    auto dictionary = [&](const uint8_t *drop) {
+        for (uint32_t sl = 0; sl < ns; sl++) {
+            std::map<std::string, int32_t> seen;
+            std::map<uint32_t, int> kseen;
+            const uint64_t a = (uint64_t)sl * rps, b = a + rps < n ? a + rps : n;
+            for (uint64_t g = a; g < b; g++) {
+                const uint8_t *aux = aux_of(g), *end = data + data_off[g + 1];
+                const uint32_t dr = drop ? drop[g] : 0u;
+                std::string line;
+                if (aux) {
+                    for (const uint8_t *p = aux; p < end;) {
+                        uint32_t vlen = 0;
+                        if (!aux_field(p, end, vlen)) break;                   // the count pass flags the record
+                        if (tb && (((dr & TAG_DROP_MD) && p[0] == 'M' && p[1] == 'D' && p[2] == 'Z') || ((dr & TAG_DROP_NM) && p[0] == 'N' && p[1] == 'M') ||
+                                   (rgv[g] >= 0 && p[0] == 'R' && p[1] == 'G' && p[2] == 'Z'))) { p += 3 + vlen; continue; }
+                        line.append((const char *)p, 3);
+                        const uint32_t key = (uint32_t)p[0] << 16 | (uint32_t)p[1] << 8 | p[2];
+                        if (!kseen.count(key)) { kseen[key] = 1; keys[sl].push_back(key); }
+                        p += 3 + vlen;
+                    }
                 }
+                auto it = seen.find(line);
+                if (it == seen.end()) { const int32_t k = (int32_t)lines[sl].size(); seen[line] = k; lines[sl].push_back(line); tl[g] = k; }
+                else tl[g] = it->second;
             }
-            auto it = seen.find(line);
-            if (it == seen.end()) { const int32_t k = (int32_t)lines[sl].size(); seen[line] = k; lines[sl].push_back(line); tl[g] = k; }
-            else tl[g] = it->second;
         }
-    }
-    // ---- device: count, scan, write ----
-    const size_t rows = (size_t)ns * S_COUNT;
+    };
+    // ---- device: the tag pass, count, scan, write ----
+    const bool tag_pass = tb && use_ref;
+    const uint32_t R = S_COUNT + (uint32_t)tkeys.size();                   // series per slice
+    const size_t rows = (size_t)ns * R;
     std::vector<uint32_t> tot(rows ? rows : 1, 0);
     std::vector<uint64_t> base(rows ? rows : 1, 0);
     std::vector<int32_t> status(n ? n : 1, 0);
@@ -409,8 +511,11 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         const auto s_ref = L.seg(ref_bytes), s_roff = L.seg(use_ref ? ((size_t)refs->n_ref + 1) * 8 : 0);
         const auto s_core = L.seg(n * 48), s_data = L.seg(data_bytes), s_doff = L.seg((n + 1) * 8), s_tl = L.seg(n * 4), s_cnt = L.seg(rows * rps * 4),
                    s_tot = L.seg(rows * 4), s_base = L.seg(rows * 8), s_st = L.seg(n * 4);
+        // tag blocks: the sorted key table, per record the tag pass's drop bits and the RG series value
+        const auto s_tkeys = L.seg(tkeys.size() * 4), s_tdrop = L.seg(tag_pass ? n : 0), s_rg = L.seg(tb ? n * 4 : 0);
         // every series byte comes from the record data, ITF8 at most 5 bytes per value: bound the arena before the scan
-        const size_t arena_cap = StageLayout::align(2 * data_bytes + 200 * n + 4096);
+        // (each tag block adds at most its 16-byte alignment)
+        const size_t arena_cap = StageLayout::align(2 * data_bytes + 200 * n + 4096 + (tb ? rows * 16 : 0));
         const auto s_arena = L.seg(arena_cap);
         // the pairing pass (mate attachment only): 2 table slots or more per read of a slice
         uint32_t tsize = 0;
@@ -424,8 +529,8 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         std::vector<uint8_t> image(L.total);
         L.base = image.data();
         memcpy(L.at(s_core), core, n * 48); memcpy(L.at(s_data), data, data_bytes); memcpy(L.at(s_doff), data_off, (n + 1) * 8);
-        memcpy(L.at(s_tl), tl.data(), n * 4);
         if (use_ref) { memcpy(L.at(s_ref), refs->bases, ref_bytes); memcpy(L.at(s_roff), refs->off, ((size_t)refs->n_ref + 1) * 8); }
+        if (tb) { memcpy(L.at(s_tkeys), tkeys.data(), tkeys.size() * 4); memcpy(L.at(s_rg), rgv.data(), n * 4); }
 #else
         if (!ctx) { hgpu_set_error("null context"); return HGPU_ERR_ARG; }
         if (cudaSetDevice(ctx->device) != cudaSuccess) return HGPU_ERR_CUDA;
@@ -433,9 +538,10 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         if (rc0) return rc0;
         cudaStream_t st = ctx->stream;
         if (hgpu_h2d(L.at(s_core), core, n * 48, st) || hgpu_h2d(L.at(s_data), data, data_bytes, st) ||
-            hgpu_h2d(L.at(s_doff), data_off, (n + 1) * 8, st) || hgpu_h2d(L.at(s_tl), tl.data(), n * 4, st)) return HGPU_ERR_CUDA;
+            hgpu_h2d(L.at(s_doff), data_off, (n + 1) * 8, st)) return HGPU_ERR_CUDA;
         if (use_ref && (hgpu_h2d(L.at(s_ref), refs->bases, ref_bytes, st) ||
                         hgpu_h2d(L.at(s_roff), refs->off, ((size_t)refs->n_ref + 1) * 8, st))) return HGPU_ERR_CUDA;
+        if (tb && (hgpu_h2d(L.at(s_tkeys), tkeys.data(), tkeys.size() * 4, st) || hgpu_h2d(L.at(s_rg), rgv.data(), n * 4, st))) return HGPU_ERR_CUDA;
 #endif
         EArgs A;
         A.core = L.at<Core>(s_core); A.data = L.at(s_data); A.data_off = L.at<uint64_t>(s_doff);
@@ -444,6 +550,10 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         A.cnt = L.at<uint32_t>(s_cnt); A.tot = L.at<uint32_t>(s_tot);
         A.base = L.at<uint64_t>(s_base); A.arena = L.at(s_arena); A.status = L.at<int32_t>(s_st);
         A.mate_cf = attach ? L.at(s_mcf) : nullptr; A.mate_nf = attach ? L.at<int32_t>(s_mnf) : nullptr;
+        A.R = R; A.tkeys = tb ? L.at<uint32_t>(s_tkeys) : nullptr; A.ntk = (uint32_t)tkeys.size();
+        A.tdrop = tag_pass ? L.at(s_tdrop) : nullptr; A.rg = tb ? L.at<int32_t>(s_rg) : nullptr;
+        TArgs TA{A.core, A.data, A.data_off, A.ref_bases, A.ref_off, A.n_ref, n, L.at(s_tdrop)};
+        std::vector<uint8_t> tdrop_h;
         PArgs P;
         P.core = A.core; P.data = A.data; P.data_off = A.data_off;
         P.ref_off = A.ref_off; P.n_ref = A.n_ref; P.no_ref = !use_ref;
@@ -453,6 +563,14 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         P.grp = L.at<int32_t>(s_grp); P.mem = L.at<uint32_t>(s_mem); P.cf = L.at(s_mcf); P.nf = L.at<int32_t>(s_mnf);
         P.hash_mask = ~0ull;
 #ifdef HGPU_HOSTSIM
+        if (tag_pass) {
+            for (uint64_t g = 0; g < n; g++) tags_body(TA, g);
+            tdrop_h.assign(TA.drop, TA.drop + n);
+        }
+        if (tb) { g_tag_drop.assign(n, 0); if (tag_pass) g_tag_drop = tdrop_h; g_tag_rg.assign(rgv.begin(), rgv.begin() + n); }
+        dictionary(tag_pass ? tdrop_h.data() : nullptr);
+        memcpy(L.at(s_tl), tl.data(), n * 4);
+        if (tb) memset(A.cnt, 0, rows * rps * 4);
         if (attach) {
             P.hash_mask = g_hash_mask;
             memset(P.slot, 0xff, slots * 4); memset(P.gcnt, 0, slots * 4); memset(P.gfill, 0, slots * 4);
@@ -468,7 +586,7 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         }
         for (uint64_t g = 0; g < n; g++) count_body(A, g);
         for (size_t row = 0; row < rows; row++) {
-            const uint64_t first = (uint64_t)(row / S_COUNT) * rps;
+            const uint64_t first = (uint64_t)(row / R) * rps;
             const uint32_t nr = (uint32_t)(n - first < rps ? n - first : rps);
             uint32_t *p = A.cnt + row * rps, run = 0;
             for (uint32_t i = 0; i < nr; i++) { const uint32_t v = p[i]; p[i] = run; run += v; }
@@ -478,13 +596,25 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         memcpy(status.data(), A.status, n * 4);
 #else
         struct Events {                                  // destroyed on every return path
-            cudaEvent_t e[6]; int n = 0;
-            bool make() { for (; n < 6; n++) if (cudaEventCreate(&e[n]) != cudaSuccess) return false; return true; }
+            cudaEvent_t e[8]; int n = 0;
+            bool make() { for (; n < 8; n++) if (cudaEventCreate(&e[n]) != cudaSuccess) return false; return true; }
             ~Events() { for (int k = 0; k < n; k++) cudaEventDestroy(e[k]); }
         } evs;
         if (!evs.make()) return HGPU_ERR_CUDA;
         cudaEvent_t *ev = evs.e;
         const unsigned rec_blocks = (unsigned)((n + 127) / 128);
+        if (tag_pass) {
+            cudaEventRecord(ev[6], st);
+            cram_enc_tags_kernel<<<rec_blocks, 128, 0, st>>>(TA);
+            cudaEventRecord(ev[7], st);
+            hgpu_count_launch();
+            if (hgpu_check(cudaGetLastError(), "cram encode tag pass launch")) return HGPU_ERR_CUDA;
+            tdrop_h.resize(n);
+            if (hgpu_d2h(tdrop_h.data(), TA.drop, n, st) || hgpu_check(cudaStreamSynchronize(st), "cram encode tag pass")) return HGPU_ERR_CUDA;
+        }
+        dictionary(tag_pass ? tdrop_h.data() : nullptr);
+        if (hgpu_h2d(L.at(s_tl), tl.data(), n * 4, st)) return HGPU_ERR_CUDA;
+        if (tb && hgpu_memset(A.cnt, 0, rows * rps * 4, st)) return HGPU_ERR_CUDA;
         cudaEventRecord(ev[0], st);
         if (attach) {
             if (hgpu_memset(P.slot, 0xff, slots * 4, st) || hgpu_memset(P.gcnt, 0, slots * 4, st) || hgpu_memset(P.gfill, 0, slots * 4, st)) return HGPU_ERR_CUDA;
@@ -534,14 +664,18 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         cudaEventElapsedTime(&cs, ev[2], ev[3]);
         cudaEventElapsedTime(&wr, ev[4], ev[5]);
         g_enc_ms[1] = cs + wr;
+        g_enc_ms[2] = 0;
+        if (tag_pass) cudaEventElapsedTime(&g_enc_ms[2], ev[6], ev[7]);
 #endif
     }
     // ---- compress the series blocks (device codecs) ----
     struct Blk { uint32_t slice; int stream; int method; std::vector<uint8_t> comp; uint32_t usize; };
     std::vector<Blk> blks;
     for (uint32_t sl = 0; sl < ns; sl++)
-        for (int s = 0; s < S_COUNT; s++)
-            if (tot[(size_t)sl * S_COUNT + s]) blks.push_back({sl, s, 0, {}, tot[(size_t)sl * S_COUNT + s]});
+        for (int s = 0; s < (int)R; s++)
+            if (tot[(size_t)sl * R + s]) blks.push_back({sl, s, 0, {}, tot[(size_t)sl * R + s]});
+    // content id: stream index + 1 for the fixed series, the tag key for a tag block
+    auto content_id = [&](int s) { return s < S_COUNT ? s + 1 : (int32_t)tkeys[(size_t)(s - S_COUNT)]; };
 #ifndef HGPU_HOSTSIM
     if (!blks.empty()) {
         // names through the tok3 encoder (CRAM 3.1); everything through the method trial; the smaller wins
@@ -554,8 +688,8 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         const uint32_t m31 = (1u << 5) | (1u << 17) | (1u << 18) | (1u << 20) | (1u << 21) | (1u << 22) | (1u << 23);    // RANS_PR0/1/64/128/129/192/193
         const uint32_t m30 = (1u << 4) | (1u << 16);                                                                  // RANS0 / RANS1
         for (uint32_t i = 0; i < nb; i++) {
-            pay[i] = arena_h.data() + base[(size_t)blks[i].slice * S_COUNT + blks[i].stream];
-            plen[i] = blks[i].usize; mask[i] = minor ? m31 : m30; cid[i] = blks[i].stream + 1;
+            pay[i] = arena_h.data() + base[(size_t)blks[i].slice * R + blks[i].stream];
+            plen[i] = blks[i].usize; mask[i] = minor ? m31 : m30; cid[i] = content_id(blks[i].stream);
             cap += (uint64_t)plen[i] + 64;
         }
         std::vector<uint8_t> framed(cap + 4096);
@@ -626,7 +760,7 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         const uint64_t a = (uint64_t)sl * rps, b = a + rps < n ? a + rps : n;
         int64_t bases = 0;
         for (uint64_t g = a; g < b; g++) bases += core[g].l_qseq;
-        Buf ch; compression_header(ch, lines[sl], keys[sl], use_ref, attach);
+        Buf ch; compression_header(ch, lines[sl], keys[sl], use_ref, attach, tb);
         Buf body;
         frame_block(body, 0, 1, 0, ch.v.data(), (uint32_t)ch.v.size(), (uint32_t)ch.v.size());
         const int32_t landmark = (int32_t)body.v.size();
@@ -636,16 +770,16 @@ int encode_impl(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, con
         Buf sh;                                                            // slice header (cram_encode_slice_header :2870)
         sh.itf8(-2); sh.itf8(0); sh.itf8(0); sh.itf8((int32_t)(b - a)); sh.ltf8((int64_t)a); sh.itf8(next + 1); sh.itf8(next + 1);
         sh.itf8(0);                                                        // content ids: the CORE block, then the external blocks
-        for (size_t k = bi; k < e; k++) sh.itf8(blks[k].stream + 1);
+        for (size_t k = bi; k < e; k++) sh.itf8(content_id(blks[k].stream));
         sh.itf8(-1);                                                       // no embedded reference
         { const uint8_t md5[16] = {0}; sh.bytes(md5, 16); }
         frame_block(body, 0, 2, 0, sh.v.data(), (uint32_t)sh.v.size(), (uint32_t)sh.v.size());
         frame_block(body, 0, 5, 0, nullptr, 0, 0);                         // CORE: every series is external
         for (size_t k = bi; k < e; k++) {
             const Blk &bk = blks[k];
-            const uint8_t *raw = arena_h.data() + base[(size_t)sl * S_COUNT + bk.stream];
-            if (bk.method == 0) frame_block(body, 0, 4, bk.stream + 1, raw, bk.usize, bk.usize);
-            else frame_block(body, bk.method, 4, bk.stream + 1, bk.comp.data(), (uint32_t)bk.comp.size(), bk.usize);
+            const uint8_t *raw = arena_h.data() + base[(size_t)sl * R + bk.stream];
+            if (bk.method == 0) frame_block(body, 0, 4, content_id(bk.stream), raw, bk.usize, bk.usize);
+            else frame_block(body, bk.method, 4, content_id(bk.stream), bk.comp.data(), (uint32_t)bk.comp.size(), bk.usize);
         }
         container(-2, 0, 0, (int32_t)(b - a), (int64_t)a, bases, next + 3, std::vector<int32_t>{landmark}, body);
         bi = e;
@@ -684,6 +818,13 @@ extern "C" uint64_t hostsim_cram_enc_mates(uint8_t *cf, int32_t *nf, uint64_t ca
     return n;
 }
 extern "C" void hostsim_cram_enc_hash_mask(uint64_t mask) { g_hash_mask = mask; }
+// test hook: the tag pass's drop bits (0 where it did not run) and the RG series values of the last call with tag blocks
+extern "C" uint64_t hostsim_cram_enc_tags(uint8_t *drop, int32_t *rg, uint64_t cap)
+{
+    const uint64_t n = g_tag_drop.size();
+    for (uint64_t i = 0; i < n && i < cap; i++) { drop[i] = g_tag_drop[i]; rg[i] = g_tag_rg[i]; }
+    return n;
+}
 #else
 extern "C" int hgpu_cram_encode_records_host(hgpu_ctx *ctx, const char *header_text, uint32_t header_len, const hgpu_bam1_core *core,
         const uint8_t *data, const uint64_t *data_off, uint64_t n, const hgpu_cram_refs *refs, uint32_t records_per_slice, int minor_version,
@@ -707,5 +848,10 @@ extern "C" void hgpu_cram_encode_last_ms(float *pair_ms, float *count_write_ms)
 {
     if (pair_ms) *pair_ms = g_enc_ms[0];
     if (count_write_ms) *count_write_ms = g_enc_ms[1];
+}
+
+extern "C" void hgpu_cram_encode_tags_last_ms(float *tag_ms)
+{
+    if (tag_ms) *tag_ms = g_enc_ms[2];
 }
 #endif

@@ -10,7 +10,8 @@
 // Series layout (all EXTERNAL, ITF8 integers; content id = stream index + 1):
 //   BF CF RI RL AP RG | RN (BYTE_ARRAY_STOP 0) | MF NS NP TS | TL | FN, per feature FC FP and DL / RS / HC / PD or
 //   BB / SC / IN (BYTE_ARRAY_LEN: length stream + value stream) | BA (unmapped reads) | QS | MQ |
-//   tags: every tag value BYTE_ARRAY_LEN over two shared streams (lengths, values), in tag-line order.
+//   tags: every tag value BYTE_ARRAY_LEN over two shared streams (lengths, values), in tag-line order; with tag blocks
+//   each tag key is a stream of its own after S_COUNT (see tag_rules / TagRec below).
 //   NF (mate distance, only with mate attachment) comes last, content id 32, so the layout without it is unchanged.
 // By default every record is written detached (MF NS NP TS explicit, no mate cross references to resolve).  With mate
 // attachment the pairing pass below decides per record, as process_one_read does, which reads of a name are attached:
@@ -76,17 +77,25 @@ CRAMREC_HD inline bool aux_field(const uint8_t *p, const uint8_t *end, uint32_t 
 }
 
 // WRITE = false: cnt[s] += bytes this record adds to stream s.  WRITE = true: the bytes go to base[s] + off[s] (off advances).
+// Streams s >= S_COUNT are the per-tag-key streams of HGPU_CRAM_ENC_TAG_BLOCKS: their counts / offsets stay in the
+// global count array (x[(s - S_COUNT) * xs], this record's column) and their bytes go to xarena + xbase[s - S_COUNT].
 template <bool WRITE>
 struct Emit {
     uint32_t *n;                     // counts or running offsets, S_COUNT entries
     uint8_t *const *base;
+    uint32_t *x = nullptr;           // tag-key streams (nullptr: none)
+    size_t xs = 0;
+    uint8_t *xarena = nullptr;
+    const uint64_t *xbase = nullptr;
+    CRAMREC_HD uint32_t &at(int s) { return s < S_COUNT ? n[s] : x[(size_t)(s - S_COUNT) * xs]; }
+    CRAMREC_HD uint8_t *dst(int s) { return s < S_COUNT ? base[s] + n[s] : xarena + xbase[s - S_COUNT] + x[(size_t)(s - S_COUNT) * xs]; }
     CRAMREC_HD void put_int(int s, int32_t v)
     {
-        if (WRITE) n[s] += (uint32_t)itf8_put(base[s] + n[s], (uint32_t)v);
-        else n[s] += (uint32_t)itf8_size((uint32_t)v);
+        if (WRITE) at(s) += (uint32_t)itf8_put(dst(s), (uint32_t)v);
+        else at(s) += (uint32_t)itf8_size((uint32_t)v);
     }
-    CRAMREC_HD void put_byte(int s, uint8_t b) { if (WRITE) base[s][n[s]] = b; n[s] += 1; }
-    CRAMREC_HD void put_bytes(int s, const uint8_t *p, uint32_t len) { if (WRITE) for (uint32_t i = 0; i < len; i++) base[s][n[s] + i] = p[i]; n[s] += len; }
+    CRAMREC_HD void put_byte(int s, uint8_t b) { if (WRITE) *dst(s) = b; at(s) += 1; }
+    CRAMREC_HD void put_bytes(int s, const uint8_t *p, uint32_t len) { if (WRITE) { uint8_t *d = dst(s); for (uint32_t i = 0; i < len; i++) d[i] = p[i]; } at(s) += len; }
     CRAMREC_HD void put_fill(int s, uint8_t b, uint32_t len) { if (WRITE) for (uint32_t i = 0; i < len; i++) base[s][n[s] + i] = b; n[s] += len; }
     CRAMREC_HD void put_bases(int s, const uint8_t *seq4, uint32_t from, uint32_t len)          // 4-bit SEQ -> ASCII
     {
@@ -166,13 +175,123 @@ CRAMREC_HD inline int features(const Core &c, const uint8_t *cig, uint32_t nc, c
     return ENC_OK;
 }
 
+// ---- tag blocks (HGPU_CRAM_ENC_TAG_BLOCKS): cram_encode_aux (cram_encode.c:2781-3200) for CRAM 3.x.  Every tag key is
+// its own series, content id = its key (tag[0] << 16 | tag[1] << 8 | type), in the byte form of the key's codec:
+// A c C s S i I f the value bytes, Z H the value with its NUL and a '\t' stop byte, B an ITF8 length and the bytes from
+// the subtype on.  An RG:Z naming an @RG line leaves the tag line, its line index goes to the RG series.  In the
+// reference-coded shape a record's MD:Z / NM are left out when the reader rebuilds them exactly (tag_rules).
+enum { TAG_DROP_MD = 1, TAG_DROP_NM = 2 };
+CRAMREC_HD inline uint32_t aux_key(const uint8_t *p) { return (uint32_t)p[0] << 16 | (uint32_t)p[1] << 8 | p[2]; }
+CRAMREC_HD inline uint8_t ascii_lower(uint8_t c) { return c >= 'A' && c <= 'Z' ? (uint8_t)(c + 32) : c; }
+
+// The MD string process_one_read would build, compared with a stored MD:Z value as strncasecmp does (:2852), one
+// character at a time as it is produced.  v == nullptr: nothing to compare with.
+struct MdCmp {
+    const uint8_t *v; uint32_t i; bool ok;
+    CRAMREC_HD void ch(uint8_t c) { if (ok && ascii_lower(v[i]) == ascii_lower(c)) i++; else ok = false; }   // v[i] == NUL never matches
+    CRAMREC_HD void num(uint64_t x)                                       // kputuw
+    {
+        uint64_t p = 1;
+        while (p <= x / 10) p *= 10;
+        for (; p; p /= 10) ch((uint8_t)('0' + x / p % 10));
+    }
+    CRAMREC_HD bool equal() const { return v && ok && v[i] == 0; }
+};
+
+// MD / NM of one record against its reference sequence (ref[0] = base 1, ref_end = its length = c->ref_end of a
+// multi-reference container, :2037-2056): process_one_read :3470-3723 and cram_encode_aux :2849-2884.  Returns the
+// TAG_DROP_* bits.  Both stay (verbatim) for an unmapped record, SEQ "*", a base 'N' in both read and reference, and a
+// match operation running past the reference end (:3512, :3525, :3605-3634); also wherever the reference's writer
+// stops with an error (CIGAR and SEQ of different lengths, a mapped read at position 0, an NM of a type it cannot read
+// whose value would have to be compared with 0).  NM is read as bam_aux2i_end reads it: c C s S i I by value, A and f
+// as 0.  Only the first MD and NM fields are looked at: the host refuses records that repeat them.
+CRAMREC_HD inline uint32_t tag_rules(const Core &c, const uint8_t *data, uint32_t l_data, const uint8_t *ref, int64_t ref_end)
+{
+    const uint32_t lq = c.l_qname, nc = c.n_cigar;
+    const int32_t ls = c.l_qseq;
+    if ((c.flag & 4) || ls <= 0 || c.pos < 0 || !ref) return 0;
+    if ((uint64_t)lq + 4ull * nc + ((uint64_t)ls + 1) / 2 + (uint64_t)ls > l_data) return 0;
+    const uint8_t *cig = data + lq, *seq4 = cig + 4 * nc, *aux = seq4 + (ls + 1) / 2 + ls, *end = data + l_data;
+    const uint8_t *md = nullptr, *nm = nullptr;
+    for (const uint8_t *p = aux; p < end;) {
+        uint32_t vlen = 0;
+        if (!aux_field(p, end, vlen)) return 0;
+        if (p[0] == 'M' && p[1] == 'D' && !md) md = p;
+        if (p[0] == 'N' && p[1] == 'M' && !nm) nm = p;
+        p += 3 + vlen;
+    }
+    if (!md && !nm) return 0;
+    MdCmp M{md && md[2] == 'Z' ? md + 3 : nullptr, 0, md && md[2] == 'Z'};
+    int64_t apos = c.pos, md_last = apos, spos = 0;
+    int32_t NM = 0;
+    for (uint32_t k = 0; k < nc; k++) {
+        const uint32_t w = cig[4 * k] | cig[4 * k + 1] << 8 | cig[4 * k + 2] << 16 | (uint32_t)cig[4 * k + 3] << 24;
+        const uint32_t op = w & 15, len = w >> 4;
+        switch (op) {
+        case 0: case 7: case 8: {
+            const int64_t e = (int64_t)len + apos < ref_end ? (int64_t)len : ref_end - apos;
+            if (e > ls || spos + (e > 0 ? e : 0) > ls) return 0;                            // the reference's writer refuses the record
+            int64_t l = 0;
+            for (; l < e; l++) {
+                const uint8_t rb = ref[apos + l], sb = base_at(seq4, (uint32_t)(spos + l));
+                if (rb == 'N' && sb == 'N') return 0;
+                if (rb != sb) { M.num((uint64_t)(apos + l - md_last)); M.ch(rb); md_last = apos + l + 1; NM++; }
+            }
+            if (l < (int64_t)len) return 0;                                                  // past the reference end
+            spos += l; apos += l;
+            break; }
+        case 2:
+            M.num((uint64_t)(apos - md_last));
+            if (apos < ref_end) {
+                M.ch('^');
+                const int64_t d = ref_end - apos < (int64_t)len ? ref_end - apos : (int64_t)len;
+                for (int64_t i = 0; i < d; i++) M.ch(ref[apos + i]);
+            }
+            NM += (int32_t)len; apos += len; md_last = apos;
+            break;
+        case 3: apos += len; md_last += len; break;
+        case 1: NM += (int32_t)len; spos += len; break;
+        case 4: spos += len; break;
+        case 5: case 6: break;
+        default: return 0;
+        }
+    }
+    if (spos != ls) return 0;
+    M.num((uint64_t)(apos - md_last));
+    uint32_t drop = M.equal() ? TAG_DROP_MD : 0;
+    if (nm) {
+        const uint8_t *v = nm + 3;
+        int32_t x;
+        switch (nm[2]) {
+        case 'c': x = (int8_t)v[0]; break;
+        case 'C': x = v[0]; break;
+        case 's': x = (int16_t)(v[0] | v[1] << 8); break;
+        case 'S': x = (int32_t)(v[0] | v[1] << 8); break;
+        case 'i': case 'I': x = (int32_t)(v[0] | v[1] << 8 | v[2] << 16 | (uint32_t)v[3] << 24); break;
+        case 'A': case 'f': x = 0; break;
+        default: x = NM == 0 ? -1 : 0; break;                                              // never equal: kept
+        }
+        if (x == NM) drop |= TAG_DROP_NM;
+    }
+    return drop;
+}
+
+// The tag-block inputs of one record (keys == nullptr: every tag value goes to the two shared streams).
+struct TagRec { const uint32_t *keys; uint32_t nkeys; uint32_t drop; int32_t rg; };
+CRAMREC_HD inline int key_stream(const TagRec &T, uint32_t key)                 // keys are sorted
+{
+    uint32_t lo = 0, hi = T.nkeys;
+    while (lo < hi) { const uint32_t m = (lo + hi) / 2; if (T.keys[m] < key) lo = m + 1; else hi = m; }
+    return lo < T.nkeys && T.keys[lo] == key ? S_COUNT + (int)lo : -1;
+}
+
 // One record.  tl = its tag-line index (the host built the dictionary).  ref / ref_len: the record's reference sequence
-// (nullptr: none).  mate_cf / mate_nf: the pairing pass's decision (MATE_DETACHED without it).  Returns ENC_OK or why
-// the slice cannot be written here.
+// (nullptr: none).  mate_cf / mate_nf: the pairing pass's decision (MATE_DETACHED without it).  T: the tag-block inputs.
+// Returns ENC_OK or why the slice cannot be written here.
 enum { MATE_DETACHED = 2, MATE_DOWNSTREAM = 4 };                               // CRAM_FLAG_DETACHED, CRAM_FLAG_MATE_DOWNSTREAM
 template <bool WRITE>
 CRAMREC_HD inline int walk(const Core &c, const uint8_t *data, uint32_t l_data, int32_t tl, const uint8_t *ref, int64_t ref_len,
-                           uint32_t mate_cf, int32_t mate_nf, Emit<WRITE> &E)
+                           uint32_t mate_cf, int32_t mate_nf, const TagRec &T, Emit<WRITE> &E)
 {
     const uint32_t lq = c.l_qname, nc = c.n_cigar;
     const int32_t ls = c.l_qseq;
@@ -198,7 +317,7 @@ CRAMREC_HD inline int walk(const Core &c, const uint8_t *data, uint32_t l_data, 
     E.put_int(S_RI, c.tid);
     E.put_int(S_RL, noseq ? (int32_t)cig_q : ls);
     E.put_int(S_AP, (int32_t)(c.pos + 1));
-    E.put_int(S_RG, -1);
+    E.put_int(S_RG, T.keys ? T.rg : -1);
     {   // the name up to its first NUL, then the stop byte
         uint32_t nl = 0;
         while (nl < lq && data[nl]) nl++;
@@ -213,13 +332,25 @@ CRAMREC_HD inline int walk(const Core &c, const uint8_t *data, uint32_t l_data, 
     }
     if (mate_cf & MATE_DOWNSTREAM) E.put_int(S_NF, mate_nf);
     E.put_int(S_TL, tl);
-    // tags: lengths + values, in order
+    // tags: lengths + values in order over two shared streams, or each value in its key's stream
     for (const uint8_t *p = aux; p < end;) {
         uint32_t vlen = 0;
         if (!aux_field(p, end, vlen)) return ENC_BAD;
-        E.put_int(S_TAG_LEN, (int32_t)vlen);
-        E.put_bytes(S_TAG_VAL, p + 3, vlen);
+        const uint8_t *v = p + 3;
+        const uint8_t t = p[2];
         p += 3 + vlen;
+        if (!T.keys) {
+            E.put_int(S_TAG_LEN, (int32_t)vlen);
+            E.put_bytes(S_TAG_VAL, v, vlen);
+            continue;
+        }
+        if (((T.drop & TAG_DROP_MD) && v[-3] == 'M' && v[-2] == 'D' && t == 'Z') || ((T.drop & TAG_DROP_NM) && v[-3] == 'N' && v[-2] == 'M') ||
+            (T.rg >= 0 && v[-3] == 'R' && v[-2] == 'G' && t == 'Z')) continue;
+        const int s = key_stream(T, aux_key(v - 3));
+        if (s < 0 || t == 'd') return ENC_UNSUPPORTED;                        // the host refuses both before the count pass
+        if (t == 'B') E.put_int(s, (int32_t)vlen);
+        E.put_bytes(s, v, vlen);
+        if (t == 'Z' || t == 'H') E.put_byte(s, '\t');
     }
     if (!unmapped) {
         uint32_t nf = 0;

@@ -522,6 +522,22 @@ int hgpu_cram_encode_records_host(hgpu_ctx *ctx, const char *header_text, uint32
  * NP / TS, and the reader rebuilds them.  Records that do not qualify stay detached.  Decided on the device by a
  * pairing pass (a name table per slice, one thread per name group) before the count pass. */
 #define HGPU_CRAM_ENC_ATTACH_MATES 0x1u
+/* HGPU_CRAM_ENC_TAG_BLOCKS: aux tags as the reference's cram_encode_aux writes them (cram/cram_encode.c:2781-3200,
+ * CRAM 3.x), combinable with HGPU_CRAM_ENC_ATTACH_MATES:
+ *   - every tag key is its own external block, content id tag[0] << 16 | tag[1] << 8 | type, with the reference's codec
+ *     for its type (BYTE_ARRAY_LEN of a one-symbol HUFFMAN length and the key's block for A c C s S i I f,
+ *     BYTE_ARRAY_STOP '\t' for Z H, BYTE_ARRAY_LEN with length and bytes in the key's block for B), instead of two
+ *     blocks shared by every tag;
+ *   - an RG:Z naming an @RG line of header_text leaves the tag line and its line index (header order) goes to the RG
+ *     series; an RG:Z naming no @RG line stays a tag;
+ *   - in the reference-coded shape only (refs cover every mapped record, RR = 1), a record's MD:Z and NM are left out
+ *     when they equal what the reader rebuilds from the reference, as process_one_read decides (:3390-3740, :2849-2884):
+ *     never for unmapped reads, SEQ "*", an 'N' in both read and reference, or a match running past the reference
+ *     end.  Without a reference they are kept, as the reference's no_ref writer keeps them.  The MD / NM decisions are
+ *     made on the device by a tag pass (one thread per record) before the count pass.
+ * Refused with HGPU_CRAM_UNSUPPORTED: an aux field of type 'd' (the reference's writer refuses it too), a record with
+ * more than one MD, NM or RG:Z field, and more than 256 distinct tag keys in one call. */
+#define HGPU_CRAM_ENC_TAG_BLOCKS 0x2u
 
 /* hgpu_cram_encode_records_host with writer options.  enc_flags = 0 gives the same bytes as
  * hgpu_cram_encode_records_host (every mate detached, no NF series in the compression header). */
@@ -531,6 +547,9 @@ int hgpu_cram_encode_records_opts_host(hgpu_ctx *ctx, const char *header_text, u
 /* measurement: device time (ms) of the last encode call's pairing kernels (0 without mate attachment) and of its
  * count + scan + write kernels */
 void hgpu_cram_encode_last_ms(float *pair_ms, float *count_write_ms);
+/* measurement: device time (ms) of the last encode call's tag pass (0 when it did not run: HGPU_CRAM_ENC_TAG_BLOCKS
+ * unset or no reference) */
+void hgpu_cram_encode_tags_last_ms(float *tag_ms);
 
 /* CRAM 3.x record decode on the device — cram_decode_slice's record loop (cram/cram_decode.c:2340-3015), cram_decode_seq
  * (:1096-1917), cram_decode_aux (:2008-2137), cram_decode_slice_xref (:2140-2304) and cram_to_bam (:3100-3211) for every
